@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the pixie_b200 hot path (contract: see the build prompt / DESIGN.md).
+"""bench.py — headline benchmark of the pixie_b200 hot path on an H100 (see DESIGN.md).
 
     python bench.py --gpus 1 --steps K --warmup W              # our arm (CUDA, through the C ABI)
+    python bench.py ... --dump-outputs DIR                     # also write the last timed step's outputs as DIR/<name>.npy
     python bench.py --impl reference --steps K --warmup W      # reference arm: the CPU path on host cores
     torchrun --nproc-per-node N ... bench.py --gpus N ...      # one rank per GPU, scenes sharded, weak scaling
 
@@ -49,15 +50,12 @@ def host_cores():
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(hbm=d["hbm_gbs"], tensor_burst=d["bf16_tflops"], tensor=d["bf16_tflops_sustained"], src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tensor_burst=1590.0, tensor=1400.0, src="fallback (B200_PROFILING.md)")
+    """Data-sheet peaks of the H100 SXM at 700 W (dense fp16 tensor rate, HBM3 bandwidth): ceilings, not measured rates."""
+    return dict(hbm=3350.0, tensor=989.0, src="H100 SXM data sheet (700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (recipe of B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index, self.rows, self.proc = index, [], None
@@ -339,8 +337,8 @@ def workload_config(args):
     return {"workload": f"configs[1]+configs[2]: U-Net seg+reg forward on one {args.grid}^3x{args.channels} fp16 voxel grid, then "
                         f"{args.substeps} MPM substeps of {args.particles} particles on a {args.mpm_grid}^3 grid; 1 scene per GPU per step",
             "parallelism": f"scene-dp{args.gpus}",
-            "l2": "U-Net input grid (268 MB) and activations exceed the 126 MB L2; the MPM working set (36 MB/substep) is "
-                  "L2-resident by construction, a 256 MB buffer is written between timed steps"}
+            "l2": "U-Net input grid (268 MB) and activations exceed the 50 MB L2; the MPM working set (36 MB/substep) fits in it, "
+                  "a 256 MB buffer is written between timed steps"}
 
 
 # ------------------------------------------------------------------------------------------------ our arm
@@ -402,6 +400,10 @@ def run_ours(args, emit):
         out_holder["seg"], out_holder["cont"] = pred.predict(feat_dev)
     ms_unet = timed(unet_step, args.steps, args.warmup)
     pred.seg_network.check(); pred.cont_network.check()
+    dumps = {}                      # --dump-outputs: what the timed paths returned in their last step
+    if args.dump_outputs and rank == 0:
+        dumps["unet_seg_logits"] = out_holder["seg"].float().cpu().numpy()
+        dumps["unet_cont"] = out_holder["cont"].float().cpu().numpy()
 
     # ---- region 2: MPM rollout, state resident; every step restarts from the same initial scene
     solver = setup_solver(sc, ng, dev)
@@ -416,6 +418,9 @@ def run_ours(args, emit):
     ms_mpm = timed(mpm_step, args.steps, args.warmup, prep=mpm_prep)
     mpm_launches_per_rollout = (solver.launch_count() - launches0) / (args.steps + args.warmup)
     x_after_rollout = solver.export_particle_x_to_torch().clone()                   # state after SUB substeps from the initial scene
+    if args.dump_outputs and rank == 0:
+        dumps["mpm_x"] = x_after_rollout.float().cpu().numpy()
+        dumps["mpm_v"] = solver.export_particle_v_to_torch().float().cpu().numpy()
     clocks = sampler.stop() if rank == 0 else None
 
     # ---- optional variants of SURVEY 8d config 3: the SVD-based plastic materials (one rollout each, after a warm-up)
@@ -483,12 +488,9 @@ def run_ours(args, emit):
             a = by.setdefault(kind, [0, 0.0, 0.0]); a[0] += 1; a[1] += ms; a[2] += fl
         conv_ms, conv_fl = by["conv"][1], by["conv"][2]
         ach = conv_fl / (conv_ms * 1e-3) * 1e-12
-        roof = {"kernel": "conv3d_igemm_kernel (tcgen05 implicit GEMM), all convolutions of seg+reg", "bound": "tensor",
-                "achieved": ach, "peak": pk["tensor"], "unit": "TFLOP/s", "frac": ach / pk["tensor"], "peak_burst": pk["tensor_burst"],
-                "peak_source": pk["src"] + ", sustained bf16",
-                # dram__bytes_read.sum + dram__bytes_write.sum of ONE dominant launch (64->64 3x3x3 @ 64^3, 58.0 GFLOP, algorithmic
-                # bytes 100.9 MB) from the committed ncu --set full capture (profiles/r01_final_summary.md section 3)
-                "traffic": 234.9e6, "traffic_launch": "128->128 3x3x3 conv @ 64^3, fp16e5 (the longest launch of a network): algorithmic 268.4e6 B (fp16 + E5M2 operands in, fp32 out), ncu dram__bytes 136.3e6 read + 98.7e6 written (profiles/r02_ncu_full_summary.md)",
+        roof = {"kernel": "conv3d_igemm_kernel (wgmma implicit GEMM), all convolutions of seg+reg", "bound": "tensor",
+                "achieved": ach, "peak": pk["tensor"], "unit": "TFLOP/s", "frac": ach / pk["tensor"],
+                "peak_source": pk["src"] + ", dense fp16",
                 "note": "achieved = algorithmic FLOPs (2*MACs of the reference graph) / sum of conv launch times from CUDA events; "
                         + {"fp16x3": "fp16x3 executes 3 fp16 tensor-core passes per algorithmic FLOP (ceiling 1/3)",
                            "fp16e5": "fp16e5 executes one fp16 pass + one E5M2 pass at twice the rate = 2 pass-equivalents per algorithmic FLOP (ceiling 1/2)",
@@ -498,7 +500,6 @@ def run_ours(args, emit):
         sub_s = ms_mpm * 1e-3 / (args.steps * SUB)
         roof_mpm = {"kernel": "mpm substep: mpm_fused_kernel (g2p + stress + p2g) + mpm_gridbox_kernel", "bound": "hbm", "achieved": per_sub_bytes / sub_s * 1e-9,
                     "peak": pk["hbm"], "unit": "GB/s", "frac": per_sub_bytes / sub_s * 1e-9 / pk["hbm"], "peak_source": pk["src"],
-                    "traffic": 8.7e6, "traffic_note": "ncu dram__bytes of mpm_fused_kernel per launch at 100k / 64^3 (8.5e6 read + 0.2e6 written): the working set is L2-resident",
                     "algorithmic_bytes_per_substep": per_sub_bytes, "us_per_substep": sub_s * 1e6}
         # counted, not estimated: the U-Net executors and the MPM handle count the kernels they enqueue (graph replays count their nodes)
         n_launch = int(round(args.steps * (pred.seg_network.launch_count() + pred.cont_network.launch_count() + mpm_launches_per_rollout)))
@@ -551,6 +552,10 @@ def run_ours(args, emit):
         dist.destroy_process_group()
     if rank != 0:
         return
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in dumps.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
     K = args.steps
     vps = world * G ** 3 * K / (ms_unet * 1e-3)
     pps = world * n * SUB * K / (ms_mpm * 1e-3)
@@ -604,6 +609,10 @@ def main():
     ap.add_argument("--skip-slab-parity", action="store_true", help="skip the decomposed-vs-undivided trajectory check at N > 1")
     ap.add_argument("--slab-slack", type=int, default=2, help="planes a particle may drift out of its slab between two migrations")
     ap.add_argument("--slab-migrate-every", type=int, default=25, help="substeps between two migration check points")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs (U-Net seg logits and material field, MPM positions "
+                         "and velocities after the rollout) to DIR/<name>.npy as float32; inputs are seeded, so runs with the same "
+                         "arguments can be compared output for output")
     ap.add_argument("--slab-lazy-trigger", type=int, default=2,
                     help="migrate only once a particle is this many planes outside its slab (0: migrate at every check point)")
     args = ap.parse_args()

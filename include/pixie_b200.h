@@ -1,4 +1,4 @@
-/* pixie_b200 — C ABI of the B200-native hot path of vlongle/pixie.
+/* pixie_b200 — C ABI of the H100-native hot path of vlongle/pixie.
  *
  * The reference has no FFI registry: its "boundary" for this path is three Python surfaces
  * (SURVEY.md §8b).  This header is what a binding of those surfaces calls; the reference-side stub a
@@ -8,7 +8,7 @@
  * and a non-zero code on failure, with a human-readable message available from pixie_last_error();
  * device pointers are BORROWED (the caller — torch in the Python shims — owns all tensors, as Warp
  * arrays alias torch memory in warp_utils.py:244-324); `stream` is a cudaStream_t passed as void*.
- * There is no CPU fallback: every entry point that computes requires an sm_100 device.
+ * There is no CPU fallback: every entry point that computes requires an sm_90 (H100) device.
  */
 #ifndef PIXIE_B200_H_
 #define PIXIE_B200_H_
@@ -22,7 +22,7 @@ extern "C" {
 const char* pixie_last_error(void);
 /* ABI version of this header (checked by the Python loader). */
 int pixie_abi_version(void);
-/* 1 if the current CUDA device is sm_100 (B200), 0 otherwise / no device. */
+/* 1 if the current CUDA device is sm_90 (H100), 0 otherwise / no device. */
 int pixie_device_ok(void);
 
 /* ===================================================================== U-Net (material field) ====

@@ -18,10 +18,9 @@ Module attribute names are the reference's, so `state_dict()` keys are identical
 reference checkpoint loads into these classes and vice versa.
 
 Pinning: the reference has no tests or golden vectors for this path (SURVEY.md §4).  This
-restatement is pinned against the reference *itself*: tests/test_oracle_unet.py imports the
-reference modules from /root/reference (when present), loads the same seeded state dict into both
-and requires bit-identical outputs; tests/golden/unet_small.npz holds input/output vectors generated
-by the reference modules with tests/golden/make_unet_golden.py for boxes without /root/reference.
+restatement is pinned against the reference *itself*: tests/golden/make_unet_golden.py runs the
+reference modules on seeded parameters and inputs, and tests/test_oracle_unet.py requires this
+restatement to reproduce their parameter names and outputs (unet_small.npz, unet_ref_modules.npz).
 """
 from __future__ import annotations
 

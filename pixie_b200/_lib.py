@@ -136,5 +136,5 @@ def check(rc: int):
 def require_device():
     lib = load()
     if not lib.pixie_device_ok():
-        raise PixieError("pixie_b200 needs an sm_100 (B200) CUDA device; there is no CPU fallback")
+        raise PixieError("pixie_b200 needs an sm_90 (H100) CUDA device; there is no CPU fallback")
     return lib

@@ -25,11 +25,11 @@ int pixie_device_ok(void) {
     if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return 0; }
     int major = 0;
     if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) { cudaGetLastError(); return 0; }
-    return major == 10 ? 1 : 0;
+    return major == 9 ? 1 : 0;
 }
 
 static int require_device() {
-    if (!pixie_device_ok()) return set_err("pixie_b200 requires an sm_100 (B200) CUDA device; there is no CPU fallback");
+    if (!pixie_device_ok()) return set_err("pixie_b200 requires an sm_90 (H100) CUDA device; there is no CPU fallback");
     return 0;
 }
 

@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM Conv3d for sm_100a: kernel + host planning. See conv3d_igemm.cuh.
+// wgmma implicit-GEMM Conv3d for sm_90a: kernel + host planning. See conv3d_igemm.cuh.
 #include "conv3d_igemm.cuh"
 #include "ptx.cuh"
 
@@ -16,61 +16,27 @@ namespace {
 
 constexpr int kMaxWStages = 2;
 constexpr int kMaxSStages = 8;
+constexpr int kConsumerWarps = 8;          // two warpgroups, 64 accumulator rows each
+constexpr int kProducerWarp = 8;
 
 struct SmemCtrl {
     uint64_t wfull[kMaxWStages];
     uint64_t wempty[kMaxWStages];
     uint64_t sfull[kMaxSStages];
     uint64_t sempty[kMaxSStages];
-    uint64_t tfull[2];
-    uint64_t tempty[2];
-    uint32_t tmem_base;
     int abort_flag;
 };
 
 constexpr int kCtlBarrierBytes = 512;     // SmemCtrl
 constexpr int kStatsMaxC = 256;
-// per epilogue warp: [2][stats_ld] floats (sum, sum of squares), private to the warp -> no atomics
-
-// Reduces v[0..15] (16 channels held by every lane = one voxel row each) over the 32 lanes of the warp.
-// Returns, in every lane, the column sum of channel stats_channel_of_lane(lane). 16 shuffles.
-__device__ __forceinline__ float warp_colsum16(float (&v)[16], int lane) {
-#pragma unroll
-    for (int half = 8, off = 16; half >= 1; half >>= 1, off >>= 1) {
-        const bool up = (lane & off) != 0;
-#pragma unroll
-        for (int i = 0; i < half; ++i) {
-            const float keep = up ? v[i + half] : v[i];
-            const float send = up ? v[i] : v[i + half];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-        }
-    }
-    return v[0] + __shfl_xor_sync(0xffffffffu, v[0], 1);
-}
-// Same for 32 channels: after the five halving steps lane l holds the column sum of channel l. 31 shuffles.
-__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
-#pragma unroll
-    for (int half = 16, off = 16; half >= 1; half >>= 1, off >>= 1) {
-        const bool up = (lane & off) != 0;
-#pragma unroll
-        for (int i = 0; i < half; ++i) {
-            const float keep = up ? v[i + half] : v[i];
-            const float send = up ? v[i] : v[i + half];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-        }
-    }
-    return v[0];
-}
-__device__ __forceinline__ int stats_channel_of_lane(int lane) {
-    return ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
-}
+// statistics rows: [2][stats_ld] floats (sum, sum of squares) shared by the consumer warps (shared-memory atomics)
 
 struct TileCoord {
     int nb, d0, h0, w0, n0, ph_begin, ph_end, split, tde;
 };
 
-// Tile coordinates of work item `wi`. On the MMA issuer's critical path once per tile (r01 trace: ~1000 cycles with signed and
-// 64-bit divisions), so: unsigned 32-bit divisions only, and none at all for the split-K bookkeeping of unsplit convolutions.
+// Tile coordinates of work item `wi`: unsigned 32-bit divisions only, and none at all for the split-K bookkeeping of
+// unsplit convolutions (this sits on the critical path of every role once per tile).
 __device__ __forceinline__ TileCoord decode_tile(const ConvKernelParams& p, int wi) {
     TileCoord t;
     unsigned rest = (unsigned)wi;
@@ -99,36 +65,75 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvKernelParams& p, int 
     return t;
 }
 
+// One (plane, kh) block: four K steps of 32 bytes (16 fp16 or 32 E5M2 values) over all BN columns, in chunks of at most 64
+// columns, as one wgmma group. Branch-free between fence and commit: ptxas serialises wgmma on any branch in between.
+template <int BN, bool F8>
+__device__ __forceinline__ void mma_block(float* acc, uint32_t a, uint32_t b) {
+    constexpr int NCH = BN < 64 ? BN : 64;
+    wgmma_fence();
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4) {
+        const uint64_t da = make_sw128_desc(a + 32u * k4);
+#pragma unroll
+        for (int s = 0; s < BN / NCH; ++s) {
+            const uint64_t db = make_sw128_desc(b + (uint32_t)(s * NCH * 128) + 32u * k4);
+            float* d = acc + s * NCH / 2;
+            if (F8) {
+                if (NCH == 16) wgmma_e5m2_n16(d, da, db);
+                if (NCH == 32) wgmma_e5m2_n32(d, da, db);
+                if (NCH == 64) wgmma_e5m2_n64(d, da, db);
+            } else {
+                if (NCH == 16) wgmma_f16_n16(d, da, db);
+                if (NCH == 32) wgmma_f16_n32(d, da, db);
+                if (NCH == 64) wgmma_f16_n64(d, da, db);
+            }
+        }
+    }
+    wgmma_commit();
+}
+
+// wgmma.wait_group with a run-time count (the instruction takes an immediate)
+__device__ __forceinline__ void wgmma_wait_n(int n) {
+    switch (n) {
+        case 0: wgmma_wait<0>(); break;
+        case 1: wgmma_wait<1>(); break;
+        case 2: wgmma_wait<2>(); break;
+        case 3: wgmma_wait<3>(); break;
+        case 4: wgmma_wait<4>(); break;
+        case 5: wgmma_wait<5>(); break;
+        case 6: wgmma_wait<6>(); break;
+        case 7: wgmma_wait<7>(); break;
+        case 8: wgmma_wait<8>(); break;
+        case 9: wgmma_wait<9>(); break;
+        default: wgmma_wait<0>(); break;
+    }
+}
+
+// One input slab (input plane pl) of a phase, for this warpgroup's 64 rows: the slab feeds output planes d = pl - kd for the
+// kd taps of the phase, each through n_kh row-shifted views (kh taps). The accumulator of plane d is acc[d]. Returns the
+// number of wgmma groups committed.
+template <int BN, int TD>
+__device__ __forceinline__ int issue_slab(float (&acc)[TD][BN / 2], uint32_t a_addr, uint32_t w_addr, int pl, int d_min, int d_max,
+                                          int n_kd, int n_kh, int TW, bool f8) {
+    int groups = 0;
+#pragma unroll
+    for (int d = 0; d < TD; ++d) {
+        if (d < d_min || d > d_max) continue;                 // warpgroup-uniform
+        const int kd = pl - d;
+        for (int kh = 0; kh < n_kh; ++kh) {
+            const uint32_t a = a_addr + (uint32_t)(kh * TW * 128);
+            const uint32_t b = w_addr + (uint32_t)((kh * n_kd + (n_kd - 1 - kd)) * BN * 128);
+            if (f8) mma_block<BN, true>(acc[d], a, b);
+            else mma_block<BN, false>(acc[d], a, b);
+            ++groups;
+        }
+    }
+    return groups;
+}
+
 }  // namespace
 
-// One input slab of a 3x3x3 stride-1 phase: 12 MMAs (3 kh x 4 K steps of 16) of N = nblk*BN columns into the nblk adjacent
-// accumulators starting at acc0. Everything that depends on (kh, k4) is a compile-time immediate so the single issuing
-// thread spends ~4 instructions per tcgen05.mma; with run-time strides it spends ~20 and becomes the kernel's bottleneck
-// (r01: 240 instructions per slab at ~7 cycles each vs 12 x 96 tensor-pipe cycles).
-template <bool F8, bool ACC>
-__device__ __forceinline__ void umma_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc) {
-    if (F8) umma_f8_lohi<ACC>(d_tmem, a_lo, b_lo, hi, idesc);
-    else umma_f16_lohi<ACC>(d_tmem, a_lo, b_lo, hi, idesc);
-}
-// (F8: the same smem geometry — 128-byte rows, four 32-byte K steps — read as E5M2 with K = 32 per instruction.)
-template <int BN, int TWv, bool F8>
-__device__ __forceinline__ void issue_slab_3x3(uint32_t acc0, uint32_t a_lo0, uint32_t b_lo0, uint32_t hi, uint32_t idA,
-                                               uint32_t id_old, uint32_t id1, int nold, bool fresh) {
-    constexpr uint32_t kKh = (uint32_t)(TWv * 128) >> 4, kTap = (uint32_t)(BN * 128) >> 4;
-    if (fresh) {
-        // the newest plane's accumulator is overwritten by its first MMA, the older planes accumulate
-        if (nold > 0) umma_lohi<F8, true>(acc0, a_lo0, b_lo0, hi, id_old);
-        umma_lohi<F8, false>(acc0 + (uint32_t)(nold * BN), a_lo0, b_lo0 + (uint32_t)nold * kTap, hi, id1);
-    } else {
-        umma_lohi<F8, true>(acc0, a_lo0, b_lo0, hi, idA);
-    }
-#pragma unroll
-    for (int i = 1; i < 12; ++i) {
-        const uint32_t kh = (uint32_t)(i >> 2), k4 = (uint32_t)(i & 3);
-        umma_lohi<F8, true>(acc0, a_lo0 + kh * kKh + 2u * k4, b_lo0 + kh * 3u * kTap + 2u * k4, hi, idA);
-    }
-}
-
+template <int BN, int TD>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -147,35 +152,27 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int total_items = p.NB * p.tiles_d * p.tiles_h * p.tiles_w * p.n_tiles * p.split_k;
-    const uint32_t tmem_cols_needed = (uint32_t)(p.acc_sets * p.TD * p.block_n);
-    uint32_t tmem_cols = 32;
-    while (tmem_cols < tmem_cols_needed) tmem_cols <<= 1;
+    const bool do_stats = p.stats != nullptr;
+    const bool scalar_stats = do_stats && p.stats_scalar;     // consumer only needs the per-item totals (LayerNorm)
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < kMaxWStages; ++i) { mbar_init(&ctl->wfull[i], 1); mbar_init(&ctl->wempty[i], 1); }
-        for (int i = 0; i < kMaxSStages; ++i) { mbar_init(&ctl->sfull[i], 1); mbar_init(&ctl->sempty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&ctl->tfull[i], 1); mbar_init(&ctl->tempty[i], 4); }
+        for (int i = 0; i < kMaxWStages; ++i) { mbar_init(&ctl->wfull[i], 1); mbar_init(&ctl->wempty[i], kConsumerWarps); }
+        for (int i = 0; i < kMaxSStages; ++i) { mbar_init(&ctl->sfull[i], 1); mbar_init(&ctl->sempty[i], kConsumerWarps); }
         ctl->abort_flag = smem_misaligned ? 1 : 0;
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(&ctl->tmem_base, tmem_cols);
-        tmem_relinquish();
-    }
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         for (int i = 0; i < kConvMaxSrc; ++i) prefetch_tmap(&p.tmA[i]);
         prefetch_tmap(&p.tmB);
     }
-    tc_fence_before();
+    if (do_stats && !scalar_stats)
+        for (int i = threadIdx.x; i < 2 * stats_ld; i += kConvThreads) stats_sm[i] = 0.f;
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = ctl->tmem_base;
     volatile int* abort_flag = &ctl->abort_flag;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         // ================================================================ TMA producer (warp-uniform, one elected lane issues)
         int ws = 0, wph = 0, ss = 0, sph = 0;
-        int wcount = 0, scount = 0;     // bring-up only (debug_flags bit 1: stop re-loading once every stage was filled)
         bool ok = true;
         for (int wi = blockIdx.x; wi < total_items && ok; wi += gridDim.x) {
             const TileCoord t = decode_tile(p, wi);
@@ -184,15 +181,13 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
                 const int ntaps = P.n_kh * P.n_kd;
                 ok = mbar_wait(&ctl->wempty[ws], wph ^ 1, abort_flag);
                 if (!ok) break;
-                if ((p.debug_flags & 2) && wcount >= p.w_stages) { if (elect_one()) mbar_arrive(&ctl->wfull[ws]); }
-                else if (elect_one()) {
+                if (elect_one()) {
                     mbar_expect_tx(&ctl->wfull[ws], (uint32_t)(ntaps * p.block_n * 128));
                     uint8_t* wdst = w_smem + (size_t)ws * p.w_stage_bytes;
                     for (int tap = 0; tap < ntaps; ++tap)
                         tma_load_2d(wdst + (size_t)tap * p.block_n * 128, &p.tmB, &ctl->wfull[ws],
                                     (P.wtile_base + tap) * 64, t.n0);
                 }
-                ++wcount;
                 if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
 
                 const int nplanes = t.tde + P.n_kd - 1;
@@ -200,140 +195,30 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
                 for (int pl = 0; pl < nplanes && ok; ++pl) {
                     ok = mbar_wait(&ctl->sempty[ss], sph ^ 1, abort_flag);
                     if (!ok) break;
-                    if ((p.debug_flags & 2) && scount >= p.s_stages) { if (elect_one()) mbar_arrive(&ctl->sfull[ss]); }
-                    else if (elect_one()) {
+                    if (elect_one()) {
                         mbar_expect_tx(&ctl->sfull[ss], slab_bytes);
                         tma_load_5d(s_smem + (size_t)ss * p.s_stage_bytes, &p.tmA[P.src],
                                     &ctl->sfull[ss], (int)P.c0, t.w0 * p.stride + P.dw,
                                     t.h0 * p.stride + P.dh0, (t.d0 + pl) * p.stride + P.dd0, t.nb);
                     }
-                    ++scount;
                     if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
                 }
             }
-        }
-    } else if (warp == 1) {
-        // ================================================================ MMA issuer
-        // The whole warp runs this loop with warp-uniform control flow (so the compiler keeps descriptors
-        // and addresses in uniform registers); only the tcgen05 instructions themselves are issued by one
-        // elected lane. A single divergent thread costs ~25 scalar instructions per MMA (ncu: tensor pipe
-        // 23 % busy, issue thread never waiting).
-        int ws = 0, wph = 0, ss = 0, sph = 0, as = 0, aph = 0;
-        const int max_blk = min(3, 256 / p.block_n);                             // accumulator blocks one MMA may span
-        const uint32_t idesc1_h = make_idesc_f16(128, (uint32_t)p.block_n), idesc2_h = make_idesc_f16(128, (uint32_t)(2 * p.block_n)),
-                       idesc3_h = make_idesc_f16(128, (uint32_t)(3 * p.block_n));
-        const uint32_t idesc1_q = make_idesc_e5m2(128, (uint32_t)p.block_n), idesc2_q = make_idesc_e5m2(128, (uint32_t)(2 * p.block_n)),
-                       idesc3_q = make_idesc_e5m2(128, (uint32_t)(3 * p.block_n));
-        const uint64_t desc_fixed = (make_sw128_desc(0, 1024) ^ p.desc_xor);   // everything but the start address
-        const uint32_t desc_lo = (uint32_t)desc_fixed, desc_hi = (uint32_t)(desc_fixed >> 32);
-        const bool fast3 = (p.block_n == 64 || p.block_n == 128) && (p.TW == 16 || p.TW == 8);
-        const uint32_t w_base0 = smem_u32(w_smem), s_base0 = smem_u32(s_smem);
-        const uint32_t kh_stride16 = (uint32_t)(p.TW * 128) >> 4;             // descriptor units of 16 B
-        const uint32_t tap_stride16 = (uint32_t)(p.block_n * 128) >> 4;
-        bool ok = true;
-        for (int wi = blockIdx.x; wi < total_items && ok; wi += gridDim.x) {
-            const TileCoord t = decode_tile(p, wi);
-            ok = mbar_wait(&ctl->tempty[as], aph ^ 1, abort_flag);
-            if (!ok) break;
-            tc_fence_after();
-            for (int ph = t.ph_begin; ph < t.ph_end && ok; ++ph) {
-                const ConvPhase P = p.phases[ph];
-                const int n_kd = P.n_kd, n_kh = P.n_kh;
-                const bool f8 = P.f8 != 0;                       // warp-uniform
-                const uint32_t idesc1 = f8 ? idesc1_q : idesc1_h, idesc2 = f8 ? idesc2_q : idesc2_h, idesc3 = f8 ? idesc3_q : idesc3_h;
-                ok = mbar_wait(&ctl->wfull[ws], wph, abort_flag);
-                if (!ok) break;
-                const uint32_t w16 = (w_base0 + (uint32_t)(ws * p.w_stage_bytes)) >> 4;
-                const int nplanes = t.tde + n_kd - 1;
-                for (int pl = 0; pl < nplanes && ok; ++pl) {
-                    ok = mbar_wait(&ctl->sfull[ss], sph, abort_flag);
-                    if (!ok) break;
-                    tc_fence_after();
-                    const uint32_t s16 = (s_base0 + (uint32_t)(ss * p.s_stage_bytes)) >> 4;
-                    // This slab (input plane pl) feeds output planes d = pl - kd: accumulators d_min..d_max are ADJACENT
-                    // column blocks of TMEM and the matching weight tiles (kd = kd_hi..kd_lo) are adjacent row blocks of
-                    // the B stage, so one MMA of N = nblk*block_n covers them all (tcgen05.mma has a ~56-cycle floor per
-                    // 128xNx16 instruction for N <= 112 and runs at N/2 cycles from N = 128 up: mma_bench.cu).
-                    const int d_min = max(0, pl - (n_kd - 1)), d_max = min(t.tde - 1, pl);
-                    const int nblk = d_max - d_min + 1, kd_hi = pl - d_min;
-                    const bool fresh = (ph == t.ph_begin) && (d_max == pl);   // plane pl's accumulator is first touched here
-                    if (elect_one()) {
-                        const uint32_t acc0 = tmem_base + (uint32_t)((as * p.TD + d_min) * p.block_n);
-                        const uint32_t wblk0 = (uint32_t)(n_kd - 1 - kd_hi);
-                        const int nold0 = fresh ? nblk - 1 : nblk;
-                        if (n_kh == 3 && n_kd == 3 && nblk <= max_blk && fast3) {
-                            const uint32_t idA = nblk == 1 ? idesc1 : (nblk == 2 ? idesc2 : idesc3);
-                            const int nold = nblk - 1;
-                            const uint32_t id_old = nold == 1 ? idesc1 : idesc2;
-                            const uint32_t a_lo0 = desc_lo | (s16 & 0x3FFFu);
-                            const uint32_t b_lo0 = desc_lo | ((w16 + wblk0 * tap_stride16) & 0x3FFFu);
-                            if (f8) {
-                                if (p.block_n == 64) {
-                                    if (p.TW == 16) issue_slab_3x3<64, 16, true>(acc0, a_lo0, b_lo0, desc_hi, idA, id_old, idesc1, nold, fresh);
-                                    else issue_slab_3x3<64, 8, true>(acc0, a_lo0, b_lo0, desc_hi, idA, id_old, idesc1, nold, fresh);
-                                } else {
-                                    if (p.TW == 16) issue_slab_3x3<128, 16, true>(acc0, a_lo0, b_lo0, desc_hi, idA, id_old, idesc1, nold, fresh);
-                                    else issue_slab_3x3<128, 8, true>(acc0, a_lo0, b_lo0, desc_hi, idA, id_old, idesc1, nold, fresh);
-                                }
-                            } else if (p.block_n == 64) {
-                                if (p.TW == 16) issue_slab_3x3<64, 16, false>(acc0, a_lo0, b_lo0, desc_hi, idA, id_old, idesc1, nold, fresh);
-                                else issue_slab_3x3<64, 8, false>(acc0, a_lo0, b_lo0, desc_hi, idA, id_old, idesc1, nold, fresh);
-                            } else {
-                                if (p.TW == 16) issue_slab_3x3<128, 16, false>(acc0, a_lo0, b_lo0, desc_hi, idA, id_old, idesc1, nold, fresh);
-                                else issue_slab_3x3<128, 8, false>(acc0, a_lo0, b_lo0, desc_hi, idA, id_old, idesc1, nold, fresh);
-                            }
-                        } else
-                        for (int kh = 0; kh < n_kh; ++kh) {
-                            const uint32_t a16 = s16 + (uint32_t)kh * kh_stride16;
-                            const uint32_t b16 = w16 + ((uint32_t)kh * (uint32_t)n_kd + wblk0) * tap_stride16;
-#pragma unroll
-                            for (int k4 = 0; k4 < 4; ++k4) {
-                                const uint64_t da = desc_fixed | (uint64_t)((a16 + 2u * k4) & 0x3FFFu);
-                                const bool split_new = fresh && kh == 0 && k4 == 0;
-                                const int nold = split_new ? nold0 : nblk;
-                                for (int b = 0; b < nold; b += max_blk) {
-                                    const int cnt = min(max_blk, nold - b);
-                                    const uint32_t idn = (cnt == 1) ? idesc1 : (cnt == 2 ? idesc2 : idesc3);
-                                    const uint64_t db = desc_fixed | (uint64_t)((b16 + (uint32_t)b * tap_stride16 + 2u * k4) & 0x3FFFu);
-                                    if (f8) umma_f8(acc0 + (uint32_t)(b * p.block_n), da, db, idn, 1u);
-                                    else umma_f16(acc0 + (uint32_t)(b * p.block_n), da, db, idn, 1u);
-                                }
-                                if (split_new) {
-                                    const uint64_t db = desc_fixed | (uint64_t)((b16 + (uint32_t)(nblk - 1) * tap_stride16 + 2u * k4) & 0x3FFFu);
-                                    if (f8) umma_f8(acc0 + (uint32_t)((nblk - 1) * p.block_n), da, db, idesc1, 0u);
-                                    else umma_f16(acc0 + (uint32_t)((nblk - 1) * p.block_n), da, db, idesc1, 0u);
-                                }
-                            }
-                        }
-                        umma_commit(&ctl->sempty[ss]);        // slab slot free once these MMAs retire
-                    }
-                    if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
-                }
-                if (elect_one()) umma_commit(&ctl->wempty[ws]);
-                if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
-            }
-            if (elect_one()) umma_commit(&ctl->tfull[as]);            // accumulators complete
-            __syncwarp();
-            if (++as == p.acc_sets) { as = 0; aph ^= 1; }
         }
     } else {
-        // ================================================================ epilogue (warps 2..5)
-        const int q = warp & 3;                 // TMEM lane quarter this warp may access
-        const int r = q * 32 + lane;            // accumulator row = voxel inside the plane tile
-        const int th = r / p.TW, tw = r % p.TW;
-        int as = 0, aph = 0;
+        // ================================================================ consumers: MMA + epilogue (warpgroups 0 and 1)
+        // Each warpgroup owns rows 64 g .. 64 g + 63 of the 128-voxel plane tile and the TD plane accumulators of those rows in
+        // registers. A slab stage is released one slab late (once only the current slab's wgmma groups are pending) so
+        // that the tensor cores always have the next slab's MMAs queued behind the current ones.
+        const int g = warp >> 2, wq = warp & 3;
+        float acc[TD][BN / 2];
+        int ws = 0, wph = 0, ss = 0, sph = 0;
+        const uint32_t w_base0 = smem_u32(w_smem), s_base0 = smem_u32(s_smem) + (uint32_t)(g * 64 * 128);
         bool ok = true;
         const long long DHW = (long long)p.D * p.H * p.W;
-        const bool do_stats = p.stats != nullptr;
-        const bool scalar_stats = do_stats && p.stats_scalar;     // consumer only needs the per-item totals (LayerNorm)
-        float* my_stats = stats_sm + (size_t)(warp - 2) * 2 * stats_ld;
-        const int et = threadIdx.x - 64;        // 0..127 among the epilogue threads
+        const int ct = threadIdx.x;             // 0..255 among the consumer threads
         int stats_nb = -1;
-        double tot_s = 0.0, tot_q = 0.0;        // scalar mode: this thread's running totals
-        if (do_stats && !scalar_stats) {
-            for (int i = lane; i < 2 * stats_ld; i += 32) my_stats[i] = 0.f;
-            __syncwarp();
-        }
+        double tot_s = 0.0, tot_q = 0.0;        // scalar statistics: this thread's running totals
         auto flush_stats = [&](int nb) {
             if (scalar_stats) {
                 // totals go to channel 0's slot; the LayerNorm consumer sums the [Cout][2] row anyway
@@ -349,255 +234,172 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
                 tot_s = 0.0; tot_q = 0.0;
                 return;
             }
-            // all 4 epilogue warps: fold the warp-private partial sums into the global fp64 accumulators
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            for (int ch = et; ch < p.Cout; ch += 128) {
-                float s = 0.f, qq = 0.f;
-#pragma unroll
-                for (int w = 0; w < 4; ++w) {
-                    s += stats_sm[(size_t)w * 2 * stats_ld + ch];
-                    qq += stats_sm[(size_t)w * 2 * stats_ld + stats_ld + ch];
-                }
-                atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2, (double)s);
-                atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2 + 1, (double)qq);
+            // both consumer warpgroups: fold the block's partial sums into the global fp64 accumulators
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            for (int ch = ct; ch < p.Cout; ch += 256) {
+                atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2, (double)stats_sm[ch]);
+                atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2 + 1, (double)stats_sm[stats_ld + ch]);
+                stats_sm[ch] = 0.f;
+                stats_sm[stats_ld + ch] = 0.f;
             }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            for (int i = lane; i < 2 * stats_ld; i += 32) my_stats[i] = 0.f;
-            __syncwarp();
+            asm volatile("bar.sync 1, 256;" ::: "memory");
         };
-        // f[0..15] = final values of 16 channels of this thread's voxel row (zero where invalid)
-        auto add_stats16 = [&](float (&f)[16], int ch0) {
-            float sq[16];
+        // accumulator rows of this thread (the two rows of the wgmma fragment)
+        int th2[2], tw2[2];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) sq[j] = f[j] * f[j];
-            if (scalar_stats) {
-                float s = 0.f, q2 = 0.f;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) { s += f[j]; q2 += sq[j]; }
-                tot_s += (double)s; tot_q += (double)q2;
-                return;
-            }
-            const float s1 = warp_colsum16(f, lane);
-            const float s2 = warp_colsum16(sq, lane);
-            const int chn = ch0 + stats_channel_of_lane(lane);
-            if ((lane & 1) == 0 && chn < p.Cout) {
-                my_stats[chn] += s1;
-                my_stats[stats_ld + chn] += s2;
-            }
-            __syncwarp();
-        };
-        const bool wide_ok = !p.out_planar && ((p.out_ld & 3) == 0) && ((p.out_c0 & 3) == 0);
-        // 256-bit accesses need 32-byte aligned rows (cudaMalloc'ed bases are 256-byte aligned)
-        const bool wide8_ok = wide_ok && ((p.out_ld & 7) == 0) && ((p.out_c0 & 7) == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 31) == 0) &&
-                              (p.residual == nullptr || (reinterpret_cast<uintptr_t>(p.residual) & 31) == 0) && !(p.debug_flags & 8);
+        for (int r2 = 0; r2 < 2; ++r2) {
+            const int r = g * 64 + wq * 16 + (lane >> 2) + 8 * r2;
+            th2[r2] = r / p.TW; tw2[r2] = r % p.TW;
+        }
+        const int cq = (lane & 3) * 2;
+
         for (int wi = blockIdx.x; wi < total_items && ok; wi += gridDim.x) {
             const TileCoord t = decode_tile(p, wi);
-            ok = mbar_wait(&ctl->tfull[as], aph, abort_flag);
+#pragma unroll
+            for (int d = 0; d < TD; ++d)
+#pragma unroll
+                for (int j = 0; j < BN / 2; ++j) acc[d][j] = 0.f;
+            int pend_s = -1, pend_w = -1;       // stages whose MMAs may still be in flight
+            int prev_f8 = -1;                   // operand type of the previous phase of this tile
+            auto release = [&]() {
+                if (lane == 0) {
+                    if (pend_s >= 0) mbar_arrive(&ctl->sempty[pend_s]);
+                    if (pend_w >= 0) mbar_arrive(&ctl->wempty[pend_w]);
+                }
+                pend_s = -1; pend_w = -1;
+            };
+            for (int ph = t.ph_begin; ph < t.ph_end && ok; ++ph) {
+                const ConvPhase P = p.phases[ph];
+                const int n_kd = P.n_kd, n_kh = P.n_kh;
+                const bool f8 = P.f8 != 0;
+                // wgmma groups of different shapes (E5M2 k32, fp16 k16) in flight on the same accumulators: drain at the switch
+                if (prev_f8 >= 0 && prev_f8 != (int)f8) wgmma_wait<0>();
+                prev_f8 = (int)f8;
+                ok = mbar_wait(&ctl->wfull[ws], wph, abort_flag);
+                if (!ok) break;
+                const uint32_t w_addr = w_base0 + (uint32_t)(ws * p.w_stage_bytes);
+                const int nplanes = t.tde + n_kd - 1;
+                for (int pl = 0; pl < nplanes && ok; ++pl) {
+                    ok = mbar_wait(&ctl->sfull[ss], sph, abort_flag);
+                    if (!ok) break;
+                    const int d_min = max(0, pl - (n_kd - 1)), d_max = min(t.tde - 1, pl);
+                    const int groups = issue_slab<BN, TD>(acc, s_base0 + (uint32_t)(ss * p.s_stage_bytes), w_addr, pl, d_min, d_max,
+                                                          n_kd, n_kh, p.TW, f8);
+                    wgmma_wait_n(groups);          // the previous slab's MMAs have retired
+                    release();
+                    pend_s = ss;
+                    if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
+                }
+                pend_w = ws;
+                if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
+                if (p.w_stages == 1) { wgmma_wait<0>(); release(); }   // the producer needs this stage for the next phase
+            }
+            wgmma_wait<0>();
+            release();
+#pragma unroll
+            for (int d = 0; d < TD; ++d)
+#pragma unroll
+                for (int j = 0; j < BN / 2; ++j) fence_operand(acc[d][j]);
             if (!ok) break;
-            tc_fence_after();
+
+            // ---------------------------------------------------------------- epilogue from registers
             if (do_stats && stats_nb != t.nb) {
                 if (stats_nb >= 0) flush_stats(stats_nb);
                 stats_nb = t.nb;
             }
-            const int hh = t.h0 + th, ww = t.w0 + tw;
-            const bool row_ok = (hh < p.H) && (ww < p.W);
             const bool first_split = (t.split == 0);
-            // ---- wide path: 32-channel chunks, chunk-outer / plane-inner, two planes in flight. One warp per scheduler means
-            // nothing hides latency but the warp's own ILP, so both TMEM loads and all residual loads are issued before
-            // the first use. Per-channel statistics are accumulated per thread over the tile's planes and reduced across
-            // the warp ONCE per (tile, chunk): the per-plane shuffle reduction cost 10 % of a 64->64 conv (r01) and its
-            // 250 shuffles per plane competed with the MMA issuer for the MIO queue.
-            int c_wide = 0;
-            if (wide_ok && !(p.debug_flags & 1)) {
-                const bool use_bias = first_split && p.bias != nullptr;
-                const bool use_res = row_ok && first_split && p.residual != nullptr;
-                const long long plane_ld = (long long)p.H * p.W * p.out_ld;
-                for (; c_wide + 32 <= p.block_n && t.n0 + c_wide + 32 <= p.Cout; c_wide += 32) {
-                    const int ch0 = t.n0 + c_wide;
-                    float cs[32], cq[32];
+            const bool use_bias = first_split && p.bias != nullptr;
+            const bool use_res = first_split && p.residual != nullptr;
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) { cs[j] = 0.f; cq[j] = 0.f; }
-                    auto finish = [&](uint32_t (&v)[32], float4 (&r)[8], long long base) {
-                        float f[32];
+            for (int d = 0; d < TD; ++d) {
+                if (d >= t.tde) break;
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
+                for (int r2 = 0; r2 < 2; ++r2) {
+                    const int hh = t.h0 + th2[r2], ww = t.w0 + tw2[r2];
+                    const bool row_ok = (hh < p.H) && (ww < p.W);
+                    const long long vox = ((long long)(t.d0 + d) * p.H + hh) * p.W + ww;   // inside batch item
+#pragma unroll
+                    for (int j8 = 0; j8 < BN / 8; ++j8) {
+                        const int ch = t.n0 + j8 * 8 + cq;
+                        float& a0 = acc[d][j8 * 4 + r2 * 2];
+                        float& a1 = acc[d][j8 * 4 + r2 * 2 + 1];
+                        const bool ok0 = row_ok && ch < p.Cout, ok1 = row_ok && ch + 1 < p.Cout;
+                        float v0 = a0, v1 = a1;
                         if (use_bias) {
-                            const float4* bp = reinterpret_cast<const float4*>(p.bias + ch0);
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const float4 b = __ldg(bp + j);
-                                f[4 * j + 0] += b.x; f[4 * j + 1] += b.y; f[4 * j + 2] += b.z; f[4 * j + 3] += b.w;
-                            }
+                            if (ok0) v0 += __ldg(p.bias + ch);
+                            if (ok1) v1 += __ldg(p.bias + ch + 1);
                         }
-                        if (use_res) {
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                f[4 * j + 0] += r[j].x; f[4 * j + 1] += r[j].y; f[4 * j + 2] += r[j].z; f[4 * j + 3] += r[j].w;
+                        if (p.out_planar) {
+                            const long long i0 = ((long long)t.nb * p.Cout + ch) * DHW + vox;
+                            if (ok0) {
+                                if (use_res) v0 += p.residual[i0];
+                                if (p.atomic_out) atomicAdd(p.out + i0, v0); else p.out[i0] = v0;
                             }
-                        }
-                        if (row_ok) {
-                            if (p.atomic_out) {
-#pragma unroll
-                                for (int j = 0; j < 8; ++j)
-                                    red_add_v4(p.out + base + 4 * j, f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-                            } else if (wide8_ok) {
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) st_global_v8(p.out + base + 8 * j, f + 8 * j);    // one full sector per store
-                            } else {
-                                float4* op = reinterpret_cast<float4*>(p.out + base);
-#pragma unroll
-                                for (int j = 0; j < 8; ++j)
-                                    op[j] = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
+                            if (ok1) {
+                                if (use_res) v1 += p.residual[i0 + DHW];
+                                if (p.atomic_out) atomicAdd(p.out + i0 + DHW, v1); else p.out[i0 + DHW] = v1;
                             }
-                            if (do_stats) {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) { cs[j] += f[j]; cq[j] = fmaf(f[j], f[j], cq[j]); }
-                            }
-                        }
-                    };
-                    for (int d = 0; d < t.tde; d += 2) {
-                        const bool two = d + 1 < t.tde;                 // warp-uniform
-                        const uint32_t acc0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)((as * p.TD + d) * p.block_n + c_wide);
-                        uint32_t v0[32], v1[32];
-                        tmem_ld32(acc0, v0);
-                        if (two) tmem_ld32(acc0 + (uint32_t)p.block_n, v1);
-                        const long long base0 = ((long long)t.nb * DHW + ((long long)(t.d0 + d) * p.H + hh) * p.W + ww) * p.out_ld + p.out_c0 + ch0;
-                        float4 r0[8], r1[8];
-                        if (use_res) {
-                            if (wide8_ok) {
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) ld_global_nc_v8(p.residual + base0 + 8 * j, reinterpret_cast<float*>(&r0[2 * j]));
-                                if (two) {
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j)
-                                        ld_global_nc_v8(p.residual + base0 + plane_ld + 8 * j, reinterpret_cast<float*>(&r1[2 * j]));
+                        } else if (ok0) {
+                            const long long base = ((long long)t.nb * DHW + vox) * p.out_ld + p.out_c0 + ch;
+                            if (ok1 && (base & 1) == 0) {
+                                if (use_res) {
+                                    const float2 rv = __ldg(reinterpret_cast<const float2*>(p.residual + base));
+                                    v0 += rv.x; v1 += rv.y;
                                 }
+                                if (p.atomic_out) red_add_v2(p.out + base, v0, v1);
+                                else *reinterpret_cast<float2*>(p.out + base) = make_float2(v0, v1);
                             } else {
-                                const float4* rp = reinterpret_cast<const float4*>(p.residual + base0);
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) r0[j] = __ldg(rp + j);
-                                if (two) {
-                                    const float4* rq = reinterpret_cast<const float4*>(p.residual + base0 + plane_ld);
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) r1[j] = __ldg(rq + j);
-                                }
+                                if (use_res) { v0 += p.residual[base]; if (ok1) v1 += p.residual[base + 1]; }
+                                if (p.atomic_out) { atomicAdd(p.out + base, v0); if (ok1) atomicAdd(p.out + base + 1, v1); }
+                                else { p.out[base] = v0; if (ok1) p.out[base + 1] = v1; }
                             }
                         }
-                        tmem_ld_wait();
-                        finish(v0, r0, base0);
-                        if (two) finish(v1, r1, base0 + plane_ld);
+                        a0 = ok0 ? v0 : 0.f;       // final values (zero where invalid) for the statistics
+                        a1 = ok1 ? v1 : 0.f;
                     }
-                    if (do_stats) {
-                        if (scalar_stats) {
+                }
+            }
+            if (do_stats) {
+                if (scalar_stats) {
+                    float s = 0.f, q2 = 0.f;
+#pragma unroll
+                    for (int d = 0; d < TD; ++d)
+#pragma unroll
+                        for (int j = 0; j < BN / 2; ++j) { s += acc[d][j]; q2 = fmaf(acc[d][j], acc[d][j], q2); }
+                    tot_s += (double)s; tot_q += (double)q2;
+                } else {
+                    // per column: this thread's rows and planes, then the 8 lanes holding the same columns
+#pragma unroll
+                    for (int j8 = 0; j8 < BN / 8; ++j8)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
                             float s = 0.f, q2 = 0.f;
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) { s += cs[j]; q2 += cq[j]; }
-                            tot_s += (double)s; tot_q += (double)q2;
-                        } else {
-                            const float s1 = warp_colsum32(cs, lane);       // lane l ends up with channel ch0 + l
-                            const float s2 = warp_colsum32(cq, lane);
-                            my_stats[ch0 + lane] += s1;
-                            my_stats[stats_ld + ch0 + lane] += s2;
-                            __syncwarp();
+                            for (int d = 0; d < TD; ++d)
+#pragma unroll
+                                for (int r2 = 0; r2 < 2; ++r2) {
+                                    const float v = acc[d][j8 * 4 + r2 * 2 + e];
+                                    s += v; q2 = fmaf(v, v, q2);
+                                }
+#pragma unroll
+                            for (int off = 4; off <= 16; off <<= 1) {
+                                s += __shfl_xor_sync(0xffffffffu, s, off);
+                                q2 += __shfl_xor_sync(0xffffffffu, q2, off);
+                            }
+                            const int ch = t.n0 + j8 * 8 + cq + e;
+                            if (lane < 4 && ch < p.Cout) {
+                                atomicAdd(stats_sm + ch, s);
+                                atomicAdd(stats_sm + stats_ld + ch, q2);
+                            }
                         }
-                    }
                 }
             }
-            for (int d = 0; d < t.tde && !(p.debug_flags & 1); ++d) {
-                const long long vox = ((long long)(t.d0 + d) * p.H + hh) * p.W + ww;   // inside batch item
-                const uint32_t acc = tmem_base + ((uint32_t)(q * 32) << 16) +
-                                     (uint32_t)((as * p.TD + d) * p.block_n);
-                int c = c_wide;
-                // ---- generic path: 16 channels per step (ragged Cout, planar outputs, narrow tiles)
-                for (; c < p.block_n; c += 16) {
-                    uint32_t v[16];
-                    tmem_ld16(acc + (uint32_t)c, v);
-                    tmem_ld_wait();
-                    const int ch0 = t.n0 + c;
-                    if (ch0 >= p.Cout) continue;              // warp-uniform
-                    float f[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]);
-                    if (first_split && p.bias) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            if (ch0 + j < p.Cout) f[j] += __ldg(p.bias + ch0 + j);
-                    }
-                    if (p.out_planar) {
-                        if (row_ok) {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) {
-                                if (ch0 + j >= p.Cout) break;
-                                const long long idx = ((long long)t.nb * p.Cout + ch0 + j) * DHW + vox;
-                                float val = f[j];
-                                if (first_split && p.residual) val += p.residual[idx];
-                                if (p.atomic_out) atomicAdd(p.out + idx, val);
-                                else p.out[idx] = val;
-                            }
-                        }
-                    } else {
-                        const long long base = ((long long)t.nb * DHW + vox) * p.out_ld + p.out_c0 + ch0;
-                        const bool vec = (ch0 + 16 <= p.Cout) && ((base & 3) == 0);
-                        if (row_ok && first_split && p.residual) {
-                            if (vec) {
-                                const float4* rp = reinterpret_cast<const float4*>(p.residual + base);
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    const float4 rv = __ldg(rp + j);
-                                    f[4 * j + 0] += rv.x; f[4 * j + 1] += rv.y;
-                                    f[4 * j + 2] += rv.z; f[4 * j + 3] += rv.w;
-                                }
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 16; ++j)
-                                    if (ch0 + j < p.Cout) f[j] += p.residual[base + j];
-                            }
-                        }
-                        if (row_ok) {
-                            if (vec) {
-                                if (p.atomic_out) {
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j)
-                                        red_add_v4(p.out + base + 4 * j, f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-                                } else {
-                                    float4* op = reinterpret_cast<float4*>(p.out + base);
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j)
-                                        op[j] = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-                                }
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 16; ++j) {
-                                    if (ch0 + j >= p.Cout) break;
-                                    if (p.atomic_out) atomicAdd(p.out + base + j, f[j]);
-                                    else p.out[base + j] = f[j];
-                                }
-                            }
-                        }
-                        if (do_stats) {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j)
-                                if (!row_ok || ch0 + j >= p.Cout) f[j] = 0.f;
-                            add_stats16(f, ch0);
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&ctl->tempty[as]);
-            if (++as == p.acc_sets) { as = 0; aph ^= 1; }
         }
         if (do_stats && stats_nb >= 0 && ok) flush_stats(stats_nb);
     }
 
-    tc_fence_before();
     __syncthreads();
     if (threadIdx.x == 0 && ctl->abort_flag && p.err_flag) atomicExch(p.err_flag, 1 + (int)blockIdx.x);
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, tmem_cols);
-    }
 }
 
 // =====================================================================================  host side
@@ -668,6 +470,10 @@ std::vector<ConvPhase> conv_build_phases(const ConvDesc& d) {
                         }
         }
     }
+    // E5M2 phases first: the tensor cores accumulate E5M2 products with a narrower mantissa than fp32, which truncates the
+    // small correction terms when they are added to accumulators already holding the fp16 partial sums; started from zero they
+    // keep their precision, and the fp16 phases then accumulate on top in full fp32. (Each phase carries its own weight tiles.)
+    std::stable_partition(ph.begin(), ph.end(), [](const ConvPhase& P) { return P.f8 != 0; });
     return ph;
 }
 
@@ -708,9 +514,8 @@ void conv_pack_weights(const ConvDesc& d, const std::vector<const float*>& seg_w
         } else if (d.stride == 1) {
             for (int c = 0; c < chunks; ++c)
                 for (int kw = 0; kw < 3; ++kw) {
-                    // tile order inside the phase: kh major, then kd = 2,1,0 — the three kd tiles of one kh are
-                    // contiguous so that ONE MMA with N = 3*block_n feeds the accumulators of output planes
-                    // p-2, p-1, p (which are adjacent TMEM column blocks)
+                    // tile order inside the phase: kh major, then kd = 2,1,0 (tile kh * 3 + 2 - kd, as the kernel's
+                    // issue_slab indexes it)
                     for (int kd = 0; kd < 3; ++kd)
                         for (int kh = 0; kh < 3; ++kh) put(wtile + kh * 3 + (2 - kd), c, kd, kh, kw);
                     wtile += 9;
@@ -721,6 +526,21 @@ void conv_pack_weights(const ConvDesc& d, const std::vector<const float*>& seg_w
                     for (int kh = 0; kh < 3; ++kh)
                         for (int kd = 0; kd < 3; ++kd) put(wtile++, c, kd, kh, kw);
         }
+    }
+}
+
+// Kernel instance for (block_n, TD); the plan guarantees a power-of-two block_n in 16..128, TD in {1, 2, 4}, TD * block_n <= 128.
+static ConvKernelFn conv_kernel_for(int bn, int td) {
+    switch (bn * 8 + td) {
+        case 16 * 8 + 1: return conv3d_igemm_kernel<16, 1>;
+        case 16 * 8 + 2: return conv3d_igemm_kernel<16, 2>;
+        case 16 * 8 + 4: return conv3d_igemm_kernel<16, 4>;
+        case 32 * 8 + 1: return conv3d_igemm_kernel<32, 1>;
+        case 32 * 8 + 2: return conv3d_igemm_kernel<32, 2>;
+        case 32 * 8 + 4: return conv3d_igemm_kernel<32, 4>;
+        case 64 * 8 + 1: return conv3d_igemm_kernel<64, 1>;
+        case 64 * 8 + 2: return conv3d_igemm_kernel<64, 2>;
+        default: return conv3d_igemm_kernel<128, 1>;
     }
 }
 
@@ -791,23 +611,30 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     bool any3 = false;
     for (const auto& P : phases) { max_taps = std::max(max_taps, P.n_kh * P.n_kd); any3 |= (P.n_kh == 3); }
 
-    // N tile
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+
+    // N tile: a power of two (16 .. 128); columns past Cout_pad are zero-filled by the weight TMA and never stored
     int bn = d.block_n;
-    if (bn == 0) bn = any3 ? std::min(64, d.Cout_pad) : std::min(256, d.Cout_pad);
-    if (bn % 16 || bn > 256 || bn < 16) return fail("bad block_n");
+    if (bn == 0) {
+        bn = 16;
+        while (bn < std::min(any3 ? 64 : 128, d.Cout_pad)) bn *= 2;
+    }
+    if (bn != 16 && bn != 32 && bn != 64 && bn != 128) return fail("bad block_n");
     p.block_n = bn;
     p.n_tiles = (d.Cout_pad + bn - 1) / bn;
 
-    // TD: accumulators per set
-    int td = d.td ? d.td : std::min(4, 512 / (2 * bn));
+    // TD: output planes per tile. Their accumulators live in the consumer warpgroups' registers: TD * block_n <= 128
+    // fp32 columns (64 registers per thread; registers are allocated per warpgroup, so 288 threads get at most 168 each).
+    int td = d.td ? d.td : std::min(4, 128 / bn);
     td = std::max(1, std::min(td, d.D));
     if (!any3) td = std::min(td, 2);    // no plane re-use without kd taps: smaller tiles, more CTAs
+    if (td == 3) td = 2;                // the kernel is instantiated for TD = 1, 2, 4
+    if (td * bn > 128) return fail("TD*block_n exceeds the register accumulator budget (128)");
     if (!d.td && td > 1) {
         // wave quantisation: a persistent grid of `sms` CTAs finishes in ceil(tiles/sms) rounds; prefer the
-        // plane count with the better last-round fill (64^3: TD=4 -> 512 tiles = 3.46 rounds, TD=2 -> 6.92)
-        int dev = 0, sms = 148;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        // plane count with the better last-round fill
         auto fill = [&](int t) {
             const long long tiles = (long long)d.NB * ((d.W + p.TW - 1) / p.TW) * ((d.H + p.TH - 1) / p.TH) * ((d.D + t - 1) / t) *
                                     ((d.Cout_pad + bn - 1) / bn);
@@ -817,8 +644,6 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
         if (fill(td / 2) > fill(td)) td /= 2;
     }
     p.TD = td;
-    p.acc_sets = (2 * td * bn <= 512) ? 2 : 1;
-    if (td * bn > 512) return fail("TD*block_n exceeds TMEM");
     p.tiles_w = (d.W + p.TW - 1) / p.TW;
     p.tiles_h = (d.H + p.TH - 1) / p.TH;
     p.tiles_d = (d.D + p.TD - 1) / p.TD;
@@ -846,7 +671,7 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     // another slab stage (the kernel then verifies the base alignment itself)
     plan.fused_stats = d.stats != nullptr && split == 1 && d.Cout <= kStatsMaxC && !d.out_planar;
     p.stats_ld = (d.Cout + 31) / 32 * 32;
-    const int stats_bytes = plan.fused_stats ? 4 * 2 * p.stats_ld * 4 : 0;
+    const int stats_bytes = plan.fused_stats ? 2 * p.stats_ld * 4 : 0;
     const int ctl_core = kCtlBarrierBytes + stats_bytes;
     auto plan_stages = [&](int slack, int& ws, int& ss) {
         const int avail = 227 * 1024 - ctl_core - slack;
@@ -868,7 +693,7 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
         const int K = conv_k_total(d);
         cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)d.Cout_pad};
         cuuint64_t gstr[1] = {(cuuint64_t)K * 2};
-        cuuint32_t box[2] = {64, (cuuint32_t)std::min(bn, d.Cout_pad)};
+        cuuint32_t box[2] = {64, (cuuint32_t)bn};
         cuuint32_t estr[2] = {1, 1};
         CUresult r = enc(&p.tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)d.weights, gdim, gstr, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -885,23 +710,14 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     p.err_flag = d_err_flag;
     p.stats = plan.fused_stats ? d.stats : nullptr;
     p.stats_scalar = d.stats_scalar ? 1 : 0;
-    p.desc_xor = 0;
-    p.debug_flags = 0;
-    if (const char* e = getenv("PIXIE_CONV_DEBUG")) p.debug_flags = atoi(e);    // bring-up A/B switches (see conv3d_igemm.cuh)
     plan.out_bytes = d.out_planar ? (size_t)d.NB * d.Cout * d.D * d.H * d.W * 4
                                   : (size_t)d.NB * d.D * d.H * d.W * p.out_ld * 4;
 
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     plan.grid = std::min(items * split, sms);
 
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(conv3d_igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-            return fail("cudaFuncSetAttribute(max dynamic smem)");
-        attr_set = true;
-    }
+    plan.kernel = conv_kernel_for(bn, td);
+    if (cudaFuncSetAttribute(plan.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+        return fail("cudaFuncSetAttribute(max dynamic smem)");
     return 0;
 }
 
@@ -916,7 +732,7 @@ int conv_plan_launch(const ConvPlan& plan, cudaStream_t stream) {
         // cleared when out_ld > Cout, so callers with sliced outputs must not use split-K.
         cudaMemsetAsync(plan.p.out, 0, plan.out_bytes, stream);
     }
-    conv3d_igemm_kernel<<<plan.grid, kConvThreads, plan.smem_bytes, stream>>>(plan.p);
+    plan.kernel<<<plan.grid, kConvThreads, plan.smem_bytes, stream>>>(plan.p);
     return (int)cudaGetLastError();
 }
 

@@ -1,4 +1,4 @@
-// Implicit-GEMM 3-D convolution on tcgen05 tensor cores (sm_100a), host-side description.
+// Implicit-GEMM 3-D convolution on Hopper tensor cores (wgmma, sm_90a), host-side description.
 //
 // Replaces, for the U-Net path, every torch.nn.Conv3d / Conv1d call of the reference
 // (third_party/Wavelet-Generation/models/module/diffusion_network.py:69-71, 91, 208-209, 571-581,
@@ -6,10 +6,12 @@
 //
 // Data layout: activations are NDHWC fp16 (the layout voxelize.py:86,111 already writes to disk),
 // weights are packed per "phase" (see below) as fp16 [Cout_pad][K] with K contiguous, accumulation
-// is fp32 in TMEM, outputs are fp32 (NDHWC, or NCDHW planar for the network head).
+// is fp32 in registers, outputs are fp32 (NDHWC, or NCDHW planar for the network head).
 //
 // GEMM view: M = output voxels (tile = TD planes x TH x TW, TH*TW = 128 rows per accumulator),
-// N = output channels (BLOCK_N <= 256 per CTA tile), K = taps x input channels in chunks of 64.
+// N = output channels (BLOCK_N <= 128 per CTA tile), K = taps x input channels in chunks of 64.
+// Each of the two consumer warpgroups computes 64 of the 128 rows for all TD planes (TD * BLOCK_N <= 128 accumulator
+// columns, 64 fp32 registers per thread) and writes them out itself; one producer warp issues the TMA loads.
 //
 // The K loop is organised in PHASES so that shared memory, not L2, serves the tap re-use:
 //   phase = (source tensor, 64-channel chunk, kw)  for 3x3x3 stride-1 convolutions.
@@ -31,7 +33,7 @@ namespace pixie {
 
 constexpr int kConvMaxSrc = 8;
 constexpr int kF8Shift = 6;        // power-of-two rebalancing between the E5M2 operands (see ConvDesc::Seg)
-constexpr int kConvThreads = 192;  // warp0 TMA, warp1 MMA, warps2-5 epilogue
+constexpr int kConvThreads = 288;  // warps 0-7: two MMA + epilogue warpgroups, warp 8: TMA producer
 
 struct ConvPhase {        // 16 bytes, lives in global memory
     int8_t src;           // tensor-map index of the activation source
@@ -42,7 +44,7 @@ struct ConvPhase {        // 16 bytes, lives in global memory
     int8_t n_kd;          // 1 or 3: kd taps served by plane marching
     int16_t c0;           // first channel of the 64-channel chunk inside the source
     int32_t wtile_base;   // index of this phase's first weight tile (64 K-columns each)
-    int32_t f8;           // 1: operands are E5M2 bytes (128 per row instead of 64 halfs), issued as kind::f8f6f4
+    int32_t f8;           // 1: operands are E5M2 bytes (128 per row instead of 64 halfs), issued as wgmma .e5m2 (K = 32)
 };
 static_assert(sizeof(ConvPhase) == 16, "ConvPhase layout");
 
@@ -55,16 +57,15 @@ struct ConvKernelParams {
     // output geometry
     int NB, D, H, W;      // batch and OUTPUT spatial size
     int stride;           // 1 or 2
-    int TW, TH, TD;       // tile: TH*TW == 128
+    int TW, TH, TD;       // tile: TH*TW == 128, TD in {1, 2, 4}
     int tiles_w, tiles_h, tiles_d;
     int Cout;             // real output channels
-    int block_n;          // N tile (multiple of 16, <= 256)
+    int block_n;          // N tile (power of two, 16 .. 128)
     int n_tiles;          // ceil(Cout / block_n)
     // shared-memory plan
     int w_stage_bytes, w_stages;   // weight stages (all taps of one phase)
     int s_stage_bytes, s_stages;   // slab stages
     int slab_rows[kConvMaxSrc];    // rows per slab for each source (TW * (TH + n_kh - 1))
-    int acc_sets;                  // 1 or 2 accumulator sets in TMEM
     // epilogue
     const float* bias;       // [Cout] or nullptr
     const float* residual;   // same layout as out, or nullptr
@@ -79,11 +80,9 @@ struct ConvKernelParams {
     int smem_slack;          // bytes reserved for aligning the dynamic smem base to 1 KB (0: the base must already be aligned)
     int stats_scalar;        // 1: only the per-item totals are wanted; they land in channel 0's slot (LayerNorm consumers)
     int* err_flag;           // device int, set non-zero on pipeline timeout
-    uint64_t desc_xor;       // bring-up only: xor into every smem matrix descriptor (0 in product use)
-    int debug_flags;         // bring-up only, timing experiments (results are WRONG when set): 1 = epilogue skips its body,
-                             // 2 = producer stops issuing TMA once every stage was filled; 8 = epilogue uses 128-bit instead of
-                             // 256-bit global accesses (results stay correct)
 };
+
+typedef void (*ConvKernelFn)(ConvKernelParams);
 
 // One activation source of a convolution.
 struct ConvSrc {
@@ -116,7 +115,7 @@ struct ConvDesc {
     double* stats = nullptr;           // request fused output statistics (honoured iff plan.fused_stats)
     bool stats_scalar = false;         // totals only (see ConvKernelParams::stats_scalar)
     int split_k = 1;                   // >1 => atomics into pre-zeroed out
-    int block_n = 0;                   // 0 = choose
+    int block_n = 0;                   // 0 = choose; else 16, 32, 64 or 128
     int td = 0;                        // 0 = choose
 };
 
@@ -135,6 +134,7 @@ void conv_pack_weights(const ConvDesc& d, const std::vector<const float*>& seg_w
 struct ConvPlan {
     ConvKernelParams p{};
     ConvPhase* d_phases = nullptr;
+    ConvKernelFn kernel = nullptr;     // instance for (block_n, TD)
     int grid = 0;
     int smem_bytes = 0;
     bool needs_zero = false;   // out must be zeroed before launch (atomic_out)

@@ -1,7 +1,6 @@
-// Standalone bring-up harness for the tcgen05 implicit-GEMM conv (not part of the product library).
+// Standalone harness for the wgmma implicit-GEMM conv (not part of the product library).
 // Runs a list of small convolutions against a CPU reference and a few large ones for timing.
 //   usage: conv_test [case-filter-substring]
-//   env:   PIXIE_DESC_XOR=<hex>   xor into the high word of every smem descriptor (bring-up only)
 #include "conv3d_igemm.cuh"
 
 #include <cuda_fp8.h>
@@ -35,8 +34,6 @@ static float frand(std::mt19937& g) { return std::uniform_real_distribution<floa
 
 int main(int argc, char** argv) {
     const char* filter = argc > 1 ? argv[1] : "";
-    uint64_t hi_xor = 0;
-    if (const char* e = getenv("PIXIE_DESC_XOR")) hi_xor = strtoull(e, nullptr, 16);
 
     std::vector<Case> cases = {
         {"gemm1x1_64_64_d16", 1, 16, 1, {64}, {64}, {{0, 1}}, 64, false, false, false, 1, 0, 0, false},
@@ -181,11 +178,9 @@ int main(int argc, char** argv) {
             ++n_fail;
             continue;
         }
-        plan.p.desc_xor = hi_xor;
-        if (getenv("CONV_DEBUG")) plan.p.debug_flags = atoi(getenv("CONV_DEBUG"));
-        printf("[%s] grid=%d smem=%d bn=%d TD=%d TW=%d TH=%d acc_sets=%d w_stages=%d s_stages=%d phases=%d split=%d\n",
+        printf("[%s] grid=%d smem=%d bn=%d TD=%d TW=%d TH=%d w_stages=%d s_stages=%d phases=%d split=%d\n",
                c.name.c_str(), plan.grid, plan.smem_bytes, plan.p.block_n, plan.p.TD, plan.p.TW, plan.p.TH,
-               plan.p.acc_sets, plan.p.w_stages, plan.p.s_stages, plan.p.n_phases, plan.p.split_k);
+               plan.p.w_stages, plan.p.s_stages, plan.p.n_phases, plan.p.split_k);
         fflush(stdout);
 
         int lrc = conv_plan_launch(plan, 0);

@@ -1,4 +1,4 @@
-// MLS-MPM / APIC substep for sm_100a.  Replaces MPM_Simulator_WARP.p2g2p
+// MLS-MPM / APIC substep for sm_90a.  Replaces MPM_Simulator_WARP.p2g2p
 // (third_party/PhysGaussian/mpm_solver_warp/mpm_solver_warp.py:514-637) and the Warp kernels it
 // launches (mpm_utils.py:295-588, BC closures mpm_solver_warp.py:785-1179).
 //
@@ -291,7 +291,7 @@ static void fused_box(Mpm* m, const float* x, long long stride_comp, long long s
     const int init[6] = {m->n_grid, m->n_grid, m->n_grid, 0, 0, 0};
     cudaMemcpyAsync(m->d_box, init, sizeof(init), cudaMemcpyHostToDevice, st);
     const float inv_dx = (float)((double)m->n_grid / (double)m->grid_lim);
-    fs_box_kernel<<<148, 256, 0, st>>>(x, stride_comp, stride_part, m->n_active, inv_dx, m->n_grid, kBoxMargin, m->d_box, 0);
+    fs_box_kernel<<<132, 256, 0, st>>>(x, stride_comp, stride_part, m->n_active, inv_dx, m->n_grid, kBoxMargin, m->d_box, 0);
     fs_box_kernel<<<1, 32, 0, st>>>(x, stride_comp, stride_part, m->n_active, inv_dx, m->n_grid, kBoxMargin, m->d_box, 1);
     m->launches += 2;
 }
@@ -419,7 +419,7 @@ static void fused_launch(Mpm* m, bool do_g2p, bool do_p2g, bool write_all, float
     FusedState t = fused_state(m);
     t.do_g2p = do_g2p; t.do_p2g = do_p2g; t.write_all = write_all;
     t.time = m->tslots + m->tpar;                 // clock of the substep whose stress / scatter runs in this launch
-    // 88 registers per thread: 32-thread blocks pack 23 per SM (736 threads), so 100k particles are one wave on 148 SMs
+    // small blocks: the fused kernel is register-heavy, and 32-thread blocks let an SM take as many as its registers allow
     static const int B = [] { const char* e = getenv("PIXIE_MPM_FUSED_BLOCK"); const int b = e ? atoi(e) : kFusedThreads; return (b == 32 || b == 64 || b == 128) ? b : kFusedThreads; }();
     const int blocks = (std::max(m->n_active, 1) + B - 1) / B;
     static const bool hoist = !(getenv("PIXIE_MPM_HOIST") && atoi(getenv("PIXIE_MPM_HOIST")) == 0);   // r02 A/B: 23.5 vs 24.1 us
@@ -797,7 +797,7 @@ int mpm_slab_excursion(Mpm* m, int* d_out, cudaStream_t st) {
     }
     const float* x = sorted ? m->fs[0].f + (size_t)FS_X * m->cap : reinterpret_cast<const float*>(m->fields[PIXIE_MPM_X]);
     if (!x) { m->error = "positions not bound"; return 1; }
-    fs_excursion_kernel<<<148, 256, 0, st>>>(x, sorted ? 1 : 3, m->n_active, inv_dx, lo, hi, d_out);
+    fs_excursion_kernel<<<132, 256, 0, st>>>(x, sorted ? 1 : 3, m->n_active, inv_dx, lo, hi, d_out);
     m->launches += 1;
     return cudaGetLastError() != cudaSuccess;
 }

@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for the sm_100a features the hot kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld).
-// Nothing here is portable: this header only compiles for sm_100a.
+// Thin inline-PTX wrappers for the sm_90a features the hot kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor) and warpgroup MMA (wgmma.mma_async).
+// Nothing here is portable: this header only compiles for sm_90a.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -55,7 +55,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded spin: a wrong descriptor must produce a failed test, not a hung GPU box.
+// Bounded spin: a wrong descriptor must produce a failed test, not a hung GPU.
 // `*abort_flag` (shared) is raised on timeout so every role in the CTA bails out.
 __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, volatile int* abort_flag) {
     for (uint32_t it = 0; it < (1u << 22); ++it) {
@@ -91,184 +91,84 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const void* tmap, uint64_
         : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc];  kind::f16 (fp16/bf16 in, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                         uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n"
-        :
-        : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// kind::f8f6f4 (8-bit float operands, K = 32 per instruction, fp32 accumulate): twice the MAC rate of kind::f16
-__device__ __forceinline__ void umma_f8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                        uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t"
-        "}\n"
-        :
-        : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-template <bool kAccumulate>
-__device__ __forceinline__ void umma_f8_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc) {
-    if (kAccumulate) {
-        asm volatile(
-            "{\n\t"
-            ".reg .b64 da, db;\n\t"
-            ".reg .pred p;\n\t"
-            "mov.b64 da, {%1, %3};\n\t"
-            "mov.b64 db, {%2, %3};\n\t"
-            "setp.eq.b32 p, 0, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], da, db, %4, p;\n\t"
-            "}\n"
-            :
-            : "r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n\t"
-            ".reg .b64 da, db;\n\t"
-            ".reg .pred p;\n\t"
-            "mov.b64 da, {%1, %3};\n\t"
-            "mov.b64 db, {%2, %3};\n\t"
-            "setp.ne.b32 p, 0, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], da, db, %4, p;\n\t"
-            "}\n"
-            :
-            : "r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc)
-            : "memory");
-    }
-}
-// Same, with the two descriptors given as (low word, shared high word): only the 14-bit start address in the low
-// word differs between operands / K steps, so the issuing thread needs one 32-bit add per operand per MMA.
-template <bool kAccumulate>
-__device__ __forceinline__ void umma_f16_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc) {
-    if (kAccumulate) {
-        asm volatile(
-            "{\n\t"
-            ".reg .b64 da, db;\n\t"
-            ".reg .pred p;\n\t"
-            "mov.b64 da, {%1, %3};\n\t"
-            "mov.b64 db, {%2, %3};\n\t"
-            "setp.eq.b32 p, 0, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t"
-            "}\n"
-            :
-            : "r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n\t"
-            ".reg .b64 da, db;\n\t"
-            ".reg .pred p;\n\t"
-            "mov.b64 da, {%1, %3};\n\t"
-            "mov.b64 db, {%2, %3};\n\t"
-            "setp.ne.b32 p, 0, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t"
-            "}\n"
-            :
-            : "r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc)
-            : "memory");
-    }
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have retired.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                     smem_u32(bar))
-                 : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread (thread i = lane i).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32"
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-          "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-          "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (r points at 32 consecutive array elements).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+// ---------------------------------------------------------------- wgmma
+// Warpgroup MMA: the 128 threads of a warpgroup compute D[64 x N] += A[64 x K] * B[N x K]^T with A and B read from shared
+// memory through matrix descriptors and D held in registers (thread t of the warpgroup owns rows 16 * (t / 32) + (t % 32) / 4
+// and that + 8, columns 8 j + 2 (t % 4) + {0, 1}: register 4 j + 2 r + e).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accesses to accumulator registers across wgmma fences and waits.
+__device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
-// K-major, 128-byte-swizzled shared-memory matrix descriptor (rows at 128 B pitch, 8-row atoms
-// of 1024 B). `sbo_bytes` = distance between consecutive 8-row atoms.
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t sbo_bytes) {
+// K-major, 128-byte-swizzled shared-memory matrix descriptor (rows at 128 B pitch, 8-row atoms of 1024 B, the layout a
+// SWIZZLE_128B TMA box writes). The start address must keep the 1024 B atom phase of the buffer, or advance inside one
+// row by a multiple of 16 B (the K steps).
+__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
     uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);         // start address   [0,14)
-    d |= static_cast<uint64_t>(1) << 16;                             // LBO (unused for SW128 K-major)
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;     // SBO             [32,46)
-    d |= static_cast<uint64_t>(1) << 46;                             // descriptor version (sm_100)
-    d |= static_cast<uint64_t>(2) << 61;                             // SWIZZLE_128B
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);   // start address         [0,14)
+    d |= static_cast<uint64_t>(1) << 16;                       // leading byte offset   (unused for SW128 K-major)
+    d |= static_cast<uint64_t>(1024 >> 4) << 32;               // stride byte offset    [32,46): 8-row atom pitch
+    d |= static_cast<uint64_t>(1) << 62;                       // layout: SWIZZLE_128B
     return d;
 }
 
-// kind::f16 instruction descriptor: A,B = fp16, D = fp32, both operands K-major, M x N tile.
-__host__ __device__ __forceinline__ uint32_t make_idesc_f16(uint32_t M, uint32_t N) {
-    return (1u << 4)            // D format: F32
-           | (0u << 7)          // A format: F16
-           | (0u << 10)         // B format: F16
-           | ((N >> 3) << 17)   // N / 8
-           | ((M >> 4) << 24);  // M / 16
+// m64nNk16 fp16 x fp16 -> fp32 and m64nNk32 E5M2 x E5M2 -> fp32, both operands K-major, D += A * B.
+__device__ __forceinline__ void wgmma_f16_n16(float* d, uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_f16_n32(float* d, uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_f16_n64(float* d, uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_e5m2_n16(float* d, uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k32.f32.e5m2.e5m2 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_e5m2_n32(float* d, uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k32.f32.e5m2.e5m2 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_e5m2_n64(float* d, uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.f32.e5m2.e5m2 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(1));
 }
 
-// kind::f8f6f4 instruction descriptor with A = B = E5M2, D = fp32, both operands K-major.
-__host__ __device__ __forceinline__ uint32_t make_idesc_e5m2(uint32_t M, uint32_t N) {
-    return (1u << 4)            // D format: F32
-           | (1u << 7)          // A format: E5M2 (E4M3 = 0)
-           | (1u << 10)         // B format: E5M2
-           | ((N >> 3) << 17)   // N / 8
-           | ((M >> 4) << 24);  // M / 16
-}
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one full 32-byte sector per thread per instruction
-__device__ __forceinline__ void st_global_v8(float* p, const float* v) {
-    asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]),
-                 "f"(v[5]), "f"(v[6]), "f"(v[7])
-                 : "memory");
-}
-__device__ __forceinline__ void ld_global_nc_v8(const float* p, float* v) {
-    asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-                 : "l"(p));
-}
 // ---------------------------------------------------------------- global red / ld helpers
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
+}
 __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b),
                  "f"(c), "f"(d)

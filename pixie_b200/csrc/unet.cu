@@ -1,5 +1,5 @@
 // U-Net executor: builds, from the reference's constructor arguments and state dict, the list of
-// kernel launches that computes SegmentationUNet / RegressionUNet.forward on one B200.
+// kernel launches that computes SegmentationUNet / RegressionUNet.forward on one H100.
 //
 // Graph restated from third_party/Wavelet-Generation/models/module/diffusion_network.py:
 //   FeatureProjector 534-589, MyResBlock 639-710, Downsample 75-97, Upsample 51-72,
@@ -178,7 +178,6 @@ struct Builder {
         d.NB = NB; d.D = d.H = d.W = sp_out; d.stride = stride; d.Cout = Cout;
         d.Cout_pad = (Cout + 15) / 16 * 16;
         d.split_k = 0;   // auto
-        if (Cout % 128 == 0 && sp_out >= 32 && !planar) d.block_n = 128;   // halves the A-slab traffic per output channel
         std::vector<const float*> wptr;
         std::vector<int> cin_real;
         std::vector<std::vector<float>> keep;

@@ -1,4 +1,4 @@
-// Memory-bound companions of the tcgen05 convolution on the U-Net path (sm_100a):
+// Memory-bound companions of the wgmma convolution on the U-Net path (sm_90a):
 //   * per-(sample, channel) moment reduction        (LayerNorm[D,H,W] / GroupNorm statistics)
 //   * normalise + affine + activation + fp16 cast   (the A operand of the next convolution)
 //   * nearest x2 upsample + fp16 cast               (diffusion_network.py:69, F.interpolate)

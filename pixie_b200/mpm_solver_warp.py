@@ -2,7 +2,7 @@
 
 Same constructor, methods, argument meaning and error behaviour as the reference class, as used by
 gs_simulation.py:68-72, 483-489, 528-531, 591-594, 634, material_field.py:232-363, 452, 531 and
-utils/decode_param.py:277-396 — but every kernel runs in libpixie_b200.so (hand-written sm_100a CUDA,
+utils/decode_param.py:277-396 — but every kernel runs in libpixie_b200.so (hand-written sm_90a CUDA,
 pixie_b200/csrc/mpm.cu) instead of Warp, substeps are replayed from a CUDA graph with the simulation
 clock on the device, and nothing synchronises with the host inside the substep loop.
 

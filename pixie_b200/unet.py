@@ -6,7 +6,7 @@ contract of
   third_party/Wavelet-Generation/trainer/training_continuous_mse.py:48-89 (RegressionUNet)
 as used by inference_combined.py:81-105 (create_models), training_utils.py:191-225
 (load_checkpoint -> load_state_dict(strict=False)) and inference_combined.py:124-126 (forward under
-torch.no_grad()).  The forward itself runs in libpixie_b200.so (tcgen05 implicit-GEMM convolutions,
+torch.no_grad()).  The forward itself runs in libpixie_b200.so (wgmma implicit-GEMM convolutions,
 see pixie_b200/csrc); PyTorch only owns the tensors and the stream.
 """
 from __future__ import annotations
@@ -116,7 +116,7 @@ class _B200UNet:
     def to(self, device):                      # create_models(...).to(rank)  (inference_combined.py:92)
         self._device = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
         if self._device.type != "cuda":
-            raise _lib.PixieError("pixie_b200 U-Net runs on CUDA (sm_100) only; there is no CPU fallback")
+            raise _lib.PixieError("pixie_b200 U-Net runs on CUDA (sm_90) only; there is no CPU fallback")
         return self
 
     def cuda(self, device=None):

@@ -1,5 +1,5 @@
-"""MPM timing A/B on the GPU box (BASELINE config 3: 100k particles, 64^3 grid): the default path with each scatter
-aggregation depth (the round-1 four-kernel path it replaced measured 46.6 us on the same box, profiles/r02_mpm_fused_first_perf.log). Usage: python scripts/gpu_mpm_perf.py [substeps]"""
+"""MPM timing A/B on the GPU (BASELINE config 3: 100k particles, 64^3 grid): the default path with each scatter
+aggregation depth. Usage: python scripts/gpu_mpm_perf.py [substeps]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

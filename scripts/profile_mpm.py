@@ -1,4 +1,4 @@
-"""Small MPM run for ncu (config 3 scene, non-graph launches). Usage: python scripts/profile_mpm.py [substeps]"""
+"""Small MPM run for a profiler (config 3 scene, non-graph launches). Usage: python scripts/profile_mpm.py [substeps]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,5 +1,5 @@
 """Two (or more) slabs of BASELINE configs[4] inside ONE process on one GPU, driven through the phase API: every flag a kernel
-waits for is already raised, so per-kernel times (ncu launch list) show the work of each slab-mode kernel without NVLink or
+waits for is already raised, so per-kernel times (profiler launch list) show the work of each slab-mode kernel without NVLink or
 waiting. usage: profile_slab_local.py [world] [substeps]"""
 import contextlib, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

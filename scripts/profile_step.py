@@ -1,4 +1,4 @@
-"""One warm-up + one measured scene (both networks, then a short MPM rollout) for ncu captures."""
+"""One warm-up + one measured scene (both networks, then a short MPM rollout) for profiler captures."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

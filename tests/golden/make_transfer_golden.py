@@ -1,5 +1,5 @@
 """Generates tests/golden/transfer_golden.npz by EXECUTING THE REFERENCE'S OWN FUNCTIONS for the steps either side of
-the two hot halves (SURVEY.md §8 f-1, f-2).  Run in the build container (the GPU box has no /root/reference):
+the two hot halves (SURVEY.md §8 f-1, f-2).  PIXIE_REFERENCE names a checkout of the reference:
 
     python tests/golden/make_transfer_golden.py
 
@@ -31,7 +31,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-REF = "/root/reference"
+REF = os.environ["PIXIE_REFERENCE"]
 PG = REF + "/third_party/PhysGaussian"
 
 import _fake_warp as wp  # noqa: E402

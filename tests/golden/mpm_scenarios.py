@@ -3,7 +3,7 @@
 A scenario is pure data: seeded particle arrays, a `set_parameters_dict` dictionary, a list of boundary-condition
 calls (method name + kwargs of the reference's `MPM_Simulator_WARP`) and checkpoints.  `replay()` drives ANY object
 with the reference's call surface through it:
-  * the reference class itself, imported from /root/reference and executed on tests/golden/_fake_warp.py
+  * the reference class itself, imported from a checkout of the reference and executed on tests/golden/_fake_warp.py
     (make_mpm_golden.py -> tests/golden/mpm_golden.npz),
   * tests/oracle_solver.OracleSolver (oracle/mpm_ref.c behind the same surface)          -> CPU test,
   * pixie_b200.mpm_solver_warp.MPM_Simulator_WARP (the CUDA path through the C ABI)       -> `-m gpu` test.

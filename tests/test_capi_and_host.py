@@ -26,7 +26,7 @@ def test_library_exports_every_header_symbol(built_lib):
 
 
 def test_no_cpu_fallback(built_lib):
-    """Without an sm_100 device every compute entry point must fail loudly."""
+    """Without an sm_90 device every compute entry point must fail loudly."""
     from pixie_b200 import _lib
     if torch.cuda.is_available():
         pytest.skip("GPU present")

@@ -1,4 +1,4 @@
-"""GPU parity tests of the U-Net path (run on the B200 box: pytest -m gpu). Every call goes through
+"""GPU parity tests of the U-Net path (needs an H100: pytest -m gpu). Every call goes through
 the C ABI (pixie_b200/_lib.py -> libpixie_b200.so); the oracle is only the checker.
 
 Tolerances (max-abs on outputs of magnitude ~3):
