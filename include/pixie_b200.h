@@ -120,6 +120,9 @@ double pixie_unet_flops(pixie_unet_t h);
 /* Test hook: copy a named intermediate fp32 activation (channels-last) to host. Names are module
  * paths of the reference ("unet.input_blocks.3.0", "projector", ...). Returns element count or <0. */
 int64_t pixie_unet_debug_fetch(pixie_unet_t h, const char* name, float* host_out, int64_t capacity);
+/* Test hook: the activations debug_fetch can copy, one "name channels side" line each, written NUL-terminated into buf.
+ * Returns the length of the full list (excluding the NUL; larger than capacity - 1 means truncated) or <0. */
+int64_t pixie_unet_debug_names(pixie_unet_t h, char* buf, int64_t capacity);
 void pixie_unet_destroy(pixie_unet_t h);
 
 /* ===================================================================== MPM (PhysGaussian rollout) =

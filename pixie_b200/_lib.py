@@ -65,6 +65,7 @@ _SIGNATURES = {
     "pixie_unet_check": (C.c_int, [C.c_void_p]),
     "pixie_unet_flops": (C.c_double, [C.c_void_p]),
     "pixie_unet_debug_fetch": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64]),
+    "pixie_unet_debug_names": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_int64]),
     "pixie_unet_destroy": (None, [C.c_void_p]),
     "pixie_mpm_create": (C.c_int, [C.c_int, C.c_int, C.c_float, C.POINTER(C.c_void_p)]),
     "pixie_mpm_bind": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),

@@ -5,6 +5,8 @@
 #include "unet_kernels.cuh"
 #include "field_transfer.cuh"
 
+#include <algorithm>
+#include <cstring>
 #include <string>
 
 namespace {
@@ -130,6 +132,16 @@ int64_t pixie_unet_debug_fetch(pixie_unet_t h, const char* name, float* host_out
     const int64_t n = pixie::unet_debug_fetch(h->u, name, host_out, capacity);
     if (n < 0) set_err(pixie::unet_error(h->u));
     return n;
+}
+int64_t pixie_unet_debug_names(pixie_unet_t h, char* buf, int64_t capacity) {
+    if (!h || (!buf && capacity > 0)) { set_err("null argument"); return -1; }
+    const std::string s = pixie::unet_debug_names(h->u);
+    if (capacity > 0) {
+        const size_t n = std::min(s.size(), (size_t)capacity - 1);
+        memcpy(buf, s.data(), n);
+        buf[n] = '\0';
+    }
+    return (int64_t)s.size();
 }
 void pixie_unet_destroy(pixie_unet_t h) {
     if (!h) return;

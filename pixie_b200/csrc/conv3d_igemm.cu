@@ -434,6 +434,7 @@ static int conv_slot_of(const std::vector<SrcSlot>& slots, int src, int n_kh) {
 
 std::vector<ConvPhase> conv_build_phases(const ConvDesc& d) {
     std::vector<ConvPhase> ph;
+    std::vector<int> rank;               // per phase: 0 E5M2 residual, 1 fp16 residual, 2 the main fp16 products
     const auto slots = conv_src_slots(d);
     int wtile = 0;
     for (const auto& s : d.segs) {
@@ -469,12 +470,18 @@ std::vector<ConvPhase> conv_build_phases(const ConvDesc& d) {
                             ph.push_back(P);
                         }
         }
+        rank.resize(ph.size(), s.f8 ? 0 : (s.lo || s.wlo) ? 1 : 2);
     }
-    // E5M2 phases first: the tensor cores accumulate E5M2 products with a narrower mantissa than fp32, which truncates the
-    // small correction terms when they are added to accumulators already holding the fp16 partial sums; started from zero they
-    // keep their precision, and the fp16 phases then accumulate on top in full fp32. (Each phase carries its own weight tiles.)
-    std::stable_partition(ph.begin(), ph.end(), [](const ConvPhase& P) { return P.f8 != 0; });
-    return ph;
+    // Residual phases first, E5M2 ones before fp16 ones: the tensor cores do not round the fp32 accumulation to nearest
+    // (and accumulate E5M2 products with a narrower mantissa still), so small correction terms added to accumulators that
+    // already hold the main partial sums lose their low bits at every K step; started from zero they keep their precision,
+    // and the main fp16 phases then accumulate on top. (Each phase carries its own weight tiles.)
+    std::vector<int> order(ph.size());
+    for (size_t i = 0; i < order.size(); ++i) order[i] = (int)i;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return rank[a] < rank[b]; });
+    std::vector<ConvPhase> sorted;
+    for (int i : order) sorted.push_back(ph[i]);
+    return sorted;
 }
 
 void conv_pack_weights(const ConvDesc& d, const std::vector<const float*>& seg_weights,
@@ -629,7 +636,7 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     // fp32 columns (64 registers per thread; registers are allocated per warpgroup, so 288 threads get at most 168 each).
     int td = d.td ? d.td : std::min(4, 128 / bn);
     td = std::max(1, std::min(td, d.D));
-    if (!any3) td = std::min(td, 2);    // no plane re-use without kd taps: smaller tiles, more CTAs
+    if (!any3 && !d.td) td = std::min(td, 2);    // no plane re-use without kd taps: smaller tiles, more CTAs (unless forced)
     if (td == 3) td = 2;                // the kernel is instantiated for TD = 1, 2, 4
     if (td * bn > 128) return fail("TD*block_n exceeds the register accumulator budget (128)");
     if (!d.td && td > 1) {
@@ -710,8 +717,8 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     p.err_flag = d_err_flag;
     p.stats = plan.fused_stats ? d.stats : nullptr;
     p.stats_scalar = d.stats_scalar ? 1 : 0;
-    plan.out_bytes = d.out_planar ? (size_t)d.NB * d.Cout * d.D * d.H * d.W * 4
-                                  : (size_t)d.NB * d.D * d.H * d.W * p.out_ld * 4;
+    plan.out_item_bytes = d.out_planar ? (size_t)d.Cout * d.D * d.H * d.W * 4
+                                       : (size_t)d.D * d.H * d.W * p.out_ld * 4;
 
     plan.grid = std::min(items * split, sms);
 
@@ -730,7 +737,9 @@ int conv_plan_launch(const ConvPlan& plan, cudaStream_t stream) {
     if (plan.needs_zero) {
         // split-K accumulates with red.add: only the channel slice written by this conv may be
         // cleared when out_ld > Cout, so callers with sliced outputs must not use split-K.
-        cudaMemsetAsync(plan.p.out, 0, plan.out_bytes, stream);
+        // Sized by the launched batch (p.NB), which callers may lower below the planned one: `out` then holds only
+        // p.NB items, and clearing the planned count would write past its end.
+        cudaMemsetAsync(plan.p.out, 0, plan.out_item_bytes * (size_t)plan.p.NB, stream);
     }
     plan.kernel<<<plan.grid, kConvThreads, plan.smem_bytes, stream>>>(plan.p);
     return (int)cudaGetLastError();

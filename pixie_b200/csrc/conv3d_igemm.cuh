@@ -103,7 +103,9 @@ struct ConvDesc {
     // e5m2(a_lo * 2^kF8Shift) followed by 64 bytes e5m2(a * 2^-kF8Shift); its weight rows hold e5m2(w * 2^-kF8Shift) followed by
     // e5m2(w_lo * 2^kF8Shift), so one K = 128-byte chunk accumulates a_lo*w + a*w_lo — the two first-order terms a single
     // fp16 pass loses — into the same fp32 accumulator (`C` of such a source counts 2-byte units like the fp16 ones).
-    struct Seg { int src; int ks; int wlo = 0; int f8 = 0; };
+    // lo = 1 marks a segment over an activation rounding residual (a_lo * w in split-precision mode). Residual segments
+    // (lo, wlo, f8) run before the others: see conv_build_phases.
+    struct Seg { int src; int ks; int wlo = 0; int f8 = 0; int lo = 0; };
     std::vector<ConvSrc> srcs;
     std::vector<Seg> segs;
     const __half* weights = nullptr;   // packed by pack_conv_weights(), [Cout_pad][K_total]
@@ -139,7 +141,7 @@ struct ConvPlan {
     int smem_bytes = 0;
     bool needs_zero = false;   // out must be zeroed before launch (atomic_out)
     bool fused_stats = false;  // the epilogue accumulates ConvDesc::stats (needs split_k == 1, Cout <= 256)
-    size_t out_bytes = 0;
+    size_t out_item_bytes = 0; // bytes of `out` per batch item; a split-K launch clears p.NB of them
 };
 
 // Returns 0 on success; on failure returns non-zero and fills `err`.

@@ -202,7 +202,7 @@ struct Builder {
                 // a_lo * w_hi  and  a_hi * w_lo
                 const int sl = (int)d.srcs.size();
                 d.srcs.push_back({in.t.lo, in.t.C, in.t.sp, in.t.sp, in.t.sp});
-                d.segs.push_back({sl, ks, 0});
+                d.segs.push_back({sl, ks, 0, 0, 1});
                 wptr.push_back(w->data.data()); cin_real.push_back(in.cin_real);
                 d.segs.push_back({si, ks, 1});
                 wptr.push_back(w->data.data()); cin_real.push_back(in.cin_real);
@@ -622,6 +622,13 @@ int64_t unet_debug_fetch(UNet* u, const char* name, float* host_out, int64_t cap
     if (check_err_flag(u)) return -4;
     cudaMemcpy(host_out, t.p, (size_t)n * 4, cudaMemcpyDeviceToHost);
     return n;
+}
+
+std::string unet_debug_names(UNet* u) {
+    std::string s;
+    for (const auto& kv : u->named)
+        s += kv.first + " " + std::to_string(kv.second.C) + " " + std::to_string(kv.second.sp) + "\n";
+    return s;
 }
 
 const std::string& unet_error(UNet* u) { return u->error; }

@@ -15,6 +15,7 @@ int unet_profile(UNet* u, const void* feat_f16, int batch, float* out, cudaStrea
 int unet_forward_ncdhw(UNet* u, const float* feat_f32, int batch, float* out, cudaStream_t st);
 int unet_forward_host(UNet* u, const void* feat_host, int batch, float* out_host, cudaStream_t st);
 int64_t unet_debug_fetch(UNet* u, const char* name, float* host_out, int64_t capacity);
+std::string unet_debug_names(UNet* u);
 const std::string& unet_error(UNet* u);
 int unet_launch_count(UNet* u);
 double unet_flops(UNet* u);

@@ -301,6 +301,21 @@ class _B200UNet:
             raise _lib.PixieError(_lib.load().pixie_last_error().decode())
         return buf[:n].view(batch, sp, sp, sp, channels).permute(0, 4, 1, 2, 3).contiguous()
 
+    def debug_names(self) -> Dict[str, Tuple[int, int]]:
+        """Activations `debug_fetch` can copy: {module path: (channels, spatial side)}."""
+        self._ensure_built()
+        lib = _lib.load()
+        n = lib.pixie_unet_debug_names(self._handle, None, 0)
+        if n < 0:
+            raise _lib.PixieError(lib.pixie_last_error().decode())
+        buf = C.create_string_buffer(n + 1)
+        lib.pixie_unet_debug_names(self._handle, buf, n + 1)
+        names = {}
+        for line in buf.value.decode().splitlines():
+            name, ch, sp = line.split()
+            names[name] = (int(ch), int(sp))
+        return names
+
 
 class SegmentationUNet(_B200UNet):
     """training_discrete.py:50-88."""

@@ -33,12 +33,52 @@ def _mine(cls_name, C, G, out, precision, sd, max_batch=2, cfg=None):
 
 
 def test_conv_bringup_binary(built_lib, cuda_dev):
-    """22 convolution shapes (1x1, 3x3x3, stride 2, concat + fused skip, split-K, planar head) against a
-    CPU double-precision reference, through the same host planner the library uses."""
+    """build/conv_test: every kernel instance, ragged and 64^3 geometry, short batches, the three statistics modes and the
+    three numerics against an fp64 host reference of the products the kernel computes, under a per-element fp32
+    accumulation bound, through the same host planner the library uses (see pixie_b200/csrc/conv_test.cu)."""
     exe = os.path.join(ROOT, "build", "conv_test")
     assert os.path.exists(exe)
-    r = subprocess.run([exe, "d"], capture_output=True, text=True, timeout=600)
-    assert "fail=0" in r.stdout, r.stdout[-3000:]
+    r = subprocess.run([exe], capture_output=True, text=True, timeout=1200)
+    summary = r.stdout[r.stdout.find("INSTANCES"):]
+    print(summary)
+    fails = [line for line in r.stdout.splitlines() if " FAIL" in line or line.startswith("FAIL")]
+    assert r.returncode == 0 and "fail=0" in r.stdout, "\n".join(fails[:40]) + "\n" + summary + r.stderr[-2000:]
+
+
+def test_unet_kernels_binary(built_lib, cuda_dev):
+    """build/unet_kernels_test: moments, norm_act, upsample2 and attention against fp64 host references, including
+    offset data, every normalisation x activation x lo layout, channel slices and logits up to +-60
+    (see pixie_b200/csrc/unet_kernels_test.cu)."""
+    exe = os.path.join(ROOT, "build", "unet_kernels_test")
+    assert os.path.exists(exe)
+    r = subprocess.run([exe], capture_output=True, text=True, timeout=600)
+    print(r.stdout[-6000:])
+    fails = [line for line in r.stdout.splitlines() if " FAIL" in line]
+    assert r.returncode == 0 and "fail=0" in r.stdout, "\n".join(fails[:40]) + r.stdout[-500:] + r.stderr[-2000:]
+
+
+@pytest.mark.parametrize("precision", ["fp16e5", "fp16x3", "fp16"])
+def test_short_batch_writes_only_the_callers_items(built_lib, cuda_dev, precision):
+    """A network built for max_batch = 2 and run on one item writes into that item only. At G = 16 the head convolution
+    uses split-K and clears its output before accumulating; the clear must cover the launched items, not max_batch of
+    them (big[1] lies right after the caller's one-item output). N = 3 runs as chunks of 2 and 1."""
+    C, G = 64, 16
+    seg, reg = O.build_pair(C, G, seed=12)
+    x = O.synthetic_features(3, C, G, seed=13)
+    with torch.no_grad():
+        refs = {"SegmentationUNet": (8, seg, seg(x)), "RegressionUNet": (3, reg, reg(x))}
+    x_cl = x.permute(0, 2, 3, 4, 1).contiguous().to(torch.float16).cuda()
+    for cls, (out, oracle, y_ref) in refs.items():
+        net = _mine(cls, C, G, out, precision, oracle.state_dict(), max_batch=2)
+        big = torch.full((2, out, G, G, G), float("nan"), device="cuda:0")
+        net.forward_channels_last_f16(x_cl[:1], out=big[:1])
+        net.check()
+        assert torch.isnan(big[1]).all(), f"{cls} {precision}: wrote past the end of a one-item output"
+        assert (big[0].cpu() - y_ref[0]).abs().max() < TOL[precision]
+        y3 = net(x.cuda()).cpu()
+        net.check()
+        for i in range(3):
+            assert (y3[i] - y_ref[i]).abs().max() < TOL[precision], (cls, i)
 
 
 @pytest.mark.parametrize("precision", ["fp16e5", "fp16x3", "fp16"])
