@@ -99,6 +99,18 @@ int pixie_knn_assign(const float* query_dev, int n_query, const float* pos_dev, 
                      float nn_distance_threshold, int weighted, const float defaults_host[4], int default_material, int default_part,
                      float* out_density_dev, float* out_E_dev, float* out_nu_dev, int* out_material_dev, int* out_part_dev,
                      float* out_conf_dev, int* n_too_far_host, void* stream);
+/* pixie_dbscan: the clustering of PG/material_field.py:365-480 (handle_stationary_clusters), scikit-learn DBSCAN semantics:
+ * over the points i of pos [n][3] with ids_dev[i] == select_id (every point when ids_dev is NULL), in index order, neighbours
+ * = fp64 squared distance <= eps^2 (self included), core = >= min_samples neighbours, clusters = connected core points labelled
+ * in the order of their smallest core index, border points take the smallest adjacent label, the rest -1.
+ * index_dev[t] = original index of the t-th selected point, labels_dev[t] = its label (both need room for n entries).
+ * *n_selected_host / *n_clusters_host receive the counts. Synchronises `stream`. */
+int pixie_dbscan(const float* pos_dev, int n, const int* ids_dev, int select_id, double eps, int min_samples, int* index_dev,
+                 int* labels_dev, int* n_selected_host, int* n_clusters_host, void* stream);
+/* pixie_cluster_stats: for the output of pixie_dbscan, per cluster the number of points (core + border) and the float32
+ * bounding box of pos over them: sizes_dev [n_clusters], bbox_min_dev / bbox_max_dev [n_clusters][3]. */
+int pixie_cluster_stats(const float* pos_dev, const int* index_dev, const int* labels_dev, int n_selected, int n_clusters,
+                        int* sizes_dev, float* bbox_min_dev, float* bbox_max_dev, void* stream);
 /* ---- either side of the substep loop (SURVEY.md 8f-2).
  * pixie_particle_volume: get_particle_volume, PG/particle_filling/filling.py:247-288 (Taichi in the reference): particles per cell
  * of a grid_n^3 grid of spacing grid_dx, vol = grid_dx^3 / count. Positions outside the grid are clamped to the border cells

@@ -89,7 +89,10 @@ _SIGNATURES = {
     "pixie_knn_assign": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                    C.c_int, C.c_float, C.c_int, C.POINTER(C.c_float), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_void_p]),
-    "pixie_particle_volume": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
+    "pixie_dbscan": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int),
+                               C.POINTER(C.c_int), C.c_void_p]),
+    "pixie_cluster_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pixie_particle_volume":(C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "pixie_frame_transform": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_float, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p]),
     "pixie_mpm_set_active_count": (C.c_int, [C.c_void_p, C.c_int]),

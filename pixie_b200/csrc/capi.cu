@@ -4,6 +4,7 @@
 #include "unet.cuh"
 #include "unet_kernels.cuh"
 #include "field_transfer.cuh"
+#include "cluster.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -97,6 +98,25 @@ int pixie_knn_assign(const float* query, int nq, const float* pos, const float* 
     if (pixie::knn_assign(query, nq, pos, density, E, nu, material, part, conf, m, k, threshold, weighted, defaults, def_material, def_part,
                           o_density, o_E, o_nu, o_material, o_part, o_conf, n_too_far_host, (cudaStream_t)stream))
         return set_err("knn_assign failed");
+    return 0;
+}
+int pixie_dbscan(const float* pos, int n, const int* ids, int select_id, double eps, int min_samples, int* index, int* labels,
+                 int* n_selected_host, int* n_clusters_host, void* stream) {
+    if (!n_selected_host || !n_clusters_host || (n > 0 && (!pos || !index || !labels))) return set_err("null argument");
+    if (n < 0) return set_err("dbscan: negative point count");
+    if (!(eps > 0.0) || min_samples < 1) return set_err("dbscan: need eps > 0 and min_samples >= 1");
+    if (require_device()) return 1;
+    if (pixie::dbscan(pos, n, ids, select_id, eps, min_samples, index, labels, n_selected_host, n_clusters_host, (cudaStream_t)stream))
+        return set_err("dbscan failed");
+    return 0;
+}
+int pixie_cluster_stats(const float* pos, const int* index, const int* labels, int n_selected, int n_clusters, int* sizes,
+                        float* bbox_min, float* bbox_max, void* stream) {
+    if (n_selected < 0 || n_clusters < 0) return set_err("cluster_stats: negative count");
+    if ((n_selected > 0 && (!pos || !index || !labels)) || (n_clusters > 0 && (!sizes || !bbox_min || !bbox_max))) return set_err("null argument");
+    if (require_device()) return 1;
+    if (pixie::cluster_stats(pos, index, labels, n_selected, n_clusters, sizes, bbox_min, bbox_max, (cudaStream_t)stream))
+        return set_err("cluster_stats failed");
     return 0;
 }
 int pixie_particle_volume(const float* pos, int n, int grid_n, float grid_dx, float* vol, void* stream) {

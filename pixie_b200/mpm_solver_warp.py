@@ -28,6 +28,8 @@ MATERIAL_ID_TO_NAME = {0: "jelly", 1: "metal", 2: "sand", 3: "visplas", 4: "flui
 EXCLUDED_MATERIAL_NAMES = ["visplas", "fluid"]
 NAME_TO_MATERIAL_ID = {name: i for i, name in MATERIAL_ID_TO_NAME.items() if name not in EXCLUDED_MATERIAL_NAMES}
 NAME_TO_MATERIAL_ID.update({"elastic": 0, "rigid": 6})
+#: boundary conditions one solver can hold (kMaxBC in csrc/mpm.cu); grid and particle BCs share the table
+MAX_BCS = 256
 
 
 def get_material_name(material_id):
@@ -149,6 +151,7 @@ class MPM_Simulator_WARP:
         m.hardening = 0.0
         m.xi = 0.0
         self._masks = []
+        self.n_bcs = 0                                   # entries used in the native BC table (MAX_BCS)
         self.grid_postprocess, self.collider_params, self.modify_bc = [], [], []
         self.pre_p2g_operations, self.impulse_params = [], []
         self.particle_velocity_modifiers, self.particle_velocity_modifier_params = [], []
@@ -407,6 +410,7 @@ class MPM_Simulator_WARP:
             self._masks.append(mask)
             bc.mask_dev = C.c_void_p(mask.data_ptr())
         _lib.check(_lib.load().pixie_mpm_add_bc(self._handle, C.byref(bc)))
+        self.n_bcs += 1
         return bc
 
     def _select_box(self, point, size) -> torch.Tensor:

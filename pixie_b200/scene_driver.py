@@ -10,7 +10,7 @@ per scene, none of it arithmetic. Here the two networks and one solver stay resi
     grid (fp16 NDHWC .npy or tensor) --predict_packed_host_stream--> (3+8, D,D,D) field     [inference_combined.py:122-199]
     field + mask --extract_material_points--> material point cloud (the PLY's vertex table)   [map_pred_to_coords.py:128-283]
     particles --get_particle_volume / load_initial_data / set_parameters_dict / BCs-->        [gs_simulation.py:464-489]
-    kNN smoothing + per-particle upload (apply_material_field_to_simulation)                  [material_field.py:295-363]
+    kNN smoothing (+ ground / stationary cuboids) + upload (apply_material_field_to_simulation) [material_field.py:295-550]
     frame loop: export positions / covariances in the Gaussians' frame, step_per_frame x p2g2p [gs_simulation.py:585-634]
 
 Function names and argument meaning follow those reference functions; rendering, Hydra and the file layout stay outside.
@@ -49,6 +49,11 @@ class Scene:
     z_shift_value: float = 0.0
     k_smoothing_neighbors: int = 10
     nn_distance_threshold: float = 0.1
+    # the ground and stationary-cluster cuboids of apply_material_field_to_simulation (material_field.py:325-336); off by
+    # default. fix_ground / only_handle_largest_cluster (decode_param.py defaults) are read only when it is on.
+    material_field_bcs: bool = False
+    fix_ground: bool = True
+    only_handle_largest_cluster: bool = True
 
 
 def transform2origin(position_tensor: torch.Tensor):
@@ -152,11 +157,18 @@ class SceneBatchDriver:
         solver.load_initial_data_from_torch(pos0, vol, cov0, n_grid=n_grid, grid_lim=grid_lim, device=str(dev))
         solver.set_parameters_dict(mp, device=str(dev))
         set_boundary_conditions(solver, sc.bc_params, tp)
-        # apply_material_field_to_simulation (material_field.py:295-341) without the DBSCAN / ground BC helpers
-        q, _ = frame_export.render_frame_transform(solver.export_particle_x_to_torch(), None, 0.0, scale_origin, original_mean_pos, rots)
-        props = material_transfer.perform_knn_smoothing(q, cloud, sc.k_smoothing_neighbors, sc.nn_distance_threshold)
-        material_transfer.apply_material_properties_to_solver(solver, props[1], props[2], props[3], props[4], device=str(dev),
-                                                              exact_box_semantics=False)
+        bc_conditions = []
+        if sc.material_field_bcs:
+            # apply_material_field_to_simulation (material_field.py:295-341): kNN, ground + stationary-cluster cuboids, upload
+            props, bc_conditions = material_transfer._apply_material_field(
+                solver, cloud, str(dev), scale_origin, original_mean_pos, rots, sc.only_handle_largest_cluster, sc.fix_ground, 0.05, 0.5,
+                sc.k_smoothing_neighbors, sc.nn_distance_threshold, False, exact_box_semantics=False)
+        else:
+            # the same without the ground / stationary-cluster BCs
+            q, _ = frame_export.render_frame_transform(solver.export_particle_x_to_torch(), None, 0.0, scale_origin, original_mean_pos, rots)
+            props = material_transfer.perform_knn_smoothing(q, cloud, sc.k_smoothing_neighbors, sc.nn_distance_threshold)
+            material_transfer.apply_material_properties_to_solver(solver, props[1], props[2], props[3], props[4], device=str(dev),
+                                                                  exact_box_semantics=False)
         substep_dt = tp["substep_dt"]
         step_per_frame = int(tp["frame_dt"] / substep_dt)                                           # float division like :627
         frames_pos, frames_cov = [], []
@@ -171,7 +183,8 @@ class SceneBatchDriver:
                 frames_cov.append(None if cr is None else cr.clone())
             solver.p2g2p_n(step_per_frame, substep_dt)
         return {"name": sc.name, "n_particles": int(pos0.shape[0]), "frames_pos": frames_pos, "frames_cov": frames_cov,
-                "material_ids": props[4], "E": props[2], "substeps": step_per_frame * int(tp["frame_num"]), "time": solver.time}
+                "material_ids": props[4], "E": props[2], "substeps": step_per_frame * int(tp["frame_num"]), "time": solver.time,
+                "bc_conditions": bc_conditions}
 
     # ------------------------------------------------------------------------------ batch
     def run(self, scenes: Sequence[Scene], out_dir: Optional[str] = None) -> List[Dict]:
