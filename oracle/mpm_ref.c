@@ -204,8 +204,20 @@ static m3 stress_dp(const m3* F, const m3* U, const m3* V, const real* sg, real 
     return m3_mul(&a, &Ft);
 }
 
+/* Branch probe of the constitutive tests (mpmref_stress_probe; NULL everywhere else). Bit b of `flip` inverts branch
+ * decision b, and margin[b] receives that decision's signed distance from its boundary, relative to the size of the
+ * compared terms (> 0: the branch is taken without the flip):
+ *   0: the plastic branch of a return map (von Mises / viscoplastic yield test, sand's dg > 0)
+ *   1: sand's tr > 0 (projection to the cone tip); the damage map's ys <= 0 after softening (mu = lam = 0) */
+typedef struct { int flip; double margin[2]; } probe_t;
+static int branch(probe_t* pr, int b, int taken, double margin) {
+    if (!pr) return taken;
+    pr->margin[b] = margin;
+    return taken ^ ((pr->flip >> b) & 1);
+}
+
 /* von_mises_return_mapping (:89-135) and ..._with_damage (:138-191) */
-static m3 return_von_mises(sim_t* s, int p, const m3* Ft, int with_damage) {
+static m3 return_von_mises(sim_t* s, int p, const m3* Ft, int with_damage, probe_t* pr) {
     m3 U, V; real so[3];
     svd3(Ft, &U, so, &V);
     real mu = s->f[F_MU][p], lam = s->f[F_LAM][p], ys = s->f[F_YIELD][p];
@@ -215,7 +227,8 @@ static m3 return_von_mises(sim_t* s, int p, const m3* Ft, int with_damage) {
     const real t0 = 2 * mu * e0 + lam * tr, t1 = 2 * mu * e1 + lam * tr, t2 = 2 * mu * e2 + lam * tr;
     const real st = t0 + t1 + t2;
     const real c0 = t0 - st / 3, c1 = t1 - st / 3, c2 = t2 - st / 3;
-    if (RSQRT(c0 * c0 + c1 * c1 + c2 * c2) > ys) {
+    const real cn = RSQRT(c0 * c0 + c1 * c1 + c2 * c2);
+    if (branch(pr, 0, cn > ys, ((double)cn - (double)ys) / ((double)cn + fabs((double)ys) + 1e-300))) {
         if (with_damage && ys <= 0) return *Ft;
         const real h0 = e0 - temp, h1 = e1 - temp, h2 = e2 - temp;
         const real hn = RSQRT(h0 * h0 + h1 * h1 + h2 * h2) + (real)1e-6;
@@ -223,9 +236,11 @@ static m3 return_von_mises(sim_t* s, int p, const m3* Ft, int with_damage) {
         const real k = dg / hn;
         e0 -= k * h0; e1 -= k * h1; e2 -= k * h2;
         if (with_damage) {
-            ys = ys - s->softening * RSQRT((k * h0) * (k * h0) + (k * h1) * (k * h1) + (k * h2) * (k * h2));
+            const real soft = s->softening * RSQRT((k * h0) * (k * h0) + (k * h1) * (k * h1) + (k * h2) * (k * h2));
+            const double scale = fabs((double)ys) + fabs((double)soft) + 1e-300;
+            ys = ys - soft;
             s->f[F_YIELD][p] = ys;
-            if (ys <= 0) { s->f[F_MU][p] = 0; s->f[F_LAM][p] = 0; }
+            if (branch(pr, 1, ys <= 0, -(double)ys / scale)) { s->f[F_MU][p] = 0; s->f[F_LAM][p] = 0; }
         }
         m3 Fe = usvt(&U, REXP(e0), REXP(e1), REXP(e2), &V);
         if (s->hardening == 1) s->f[F_YIELD][p] = s->f[F_YIELD][p] + 2 * s->f[F_MU][p] * s->xi * dg;
@@ -234,7 +249,7 @@ static m3 return_von_mises(sim_t* s, int p, const m3* Ft, int with_damage) {
     return *Ft;
 }
 /* viscoplasticity_return_mapping_with_StVK, :195-239 */
-static m3 return_viscoplastic(sim_t* s, int p, const m3* Ft, real dt) {
+static m3 return_viscoplastic(sim_t* s, int p, const m3* Ft, real dt, probe_t* pr) {
     m3 U, V; real so[3];
     svd3(Ft, &U, so, &V);
     const real mu = s->f[F_MU][p];
@@ -244,8 +259,9 @@ static m3 return_viscoplastic(sim_t* s, int p, const m3* Ft, real dt) {
     const real h0 = e0 - tr / 3, h1 = e1 - tr / 3, h2 = e2 - tr / 3;
     const real s0 = 2 * mu * h0, s1 = 2 * mu * h1, s2 = 2 * mu * h2;
     const real sn = RSQRT(s0 * s0 + s1 * s1 + s2 * s2);
-    const real y = sn - RSQRT((real)2 / (real)3) * s->f[F_YIELD][p];
-    if (y > 0) {
+    const real yt = RSQRT((real)2 / (real)3) * s->f[F_YIELD][p];
+    const real y = sn - yt;
+    if (branch(pr, 0, y > 0, (double)y / ((double)sn + fabs((double)yt) + 1e-300))) {
         const real mu_hat = mu * (b0 + b1 + b2) / 3;
         const real snew = sn - y / (1 + s->plastic_viscosity / (2 * mu_hat * dt));
         const real r = snew / sn, k = 1 / (2 * mu);
@@ -254,7 +270,7 @@ static m3 return_viscoplastic(sim_t* s, int p, const m3* Ft, real dt) {
     return *Ft;
 }
 /* sand_return_mapping, :242-279 */
-static m3 return_sand(sim_t* s, int p, const m3* Ft) {
+static m3 return_sand(sim_t* s, int p, const m3* Ft, probe_t* pr) {
     m3 U, V; real sg[3];
     svd3(Ft, &U, sg, &V);
     const real mu = s->f[F_MU][p], lam = s->f[F_LAM][p];
@@ -263,23 +279,27 @@ static m3 return_sand(sim_t* s, int p, const m3* Ft) {
     const real tr = e0 + e1 + e2;
     const real h0 = e0 - tr / 3, h1 = e1 - tr / 3, h2 = e2 - tr / 3;
     const real hn = RSQRT(h0 * h0 + h1 * h1 + h2 * h2);
-    const real dg = hn + (3 * lam + 2 * mu) / (2 * mu) * tr * s->alpha;
-    if (dg <= 0) return *Ft;
-    if (tr > 0) { m3 Vt = m3_t(&V); return m3_mul(&U, &Vt); }
+    const real cone = (3 * lam + 2 * mu) / (2 * mu) * tr * s->alpha;
+    const real dg = hn + cone;
+    if (!branch(pr, 0, dg > 0, (double)dg / ((double)hn + fabs((double)cone) + 1e-300))) return *Ft;
+    if (branch(pr, 1, tr > 0, (double)tr / (fabs((double)e0) + fabs((double)e1) + fabs((double)e2) + 1e-300))) {
+        m3 Vt = m3_t(&V);
+        return m3_mul(&U, &Vt);
+    }
     const real k = dg / hn;
     return usvt(&U, REXP(e0 - h0 * k), REXP(e1 - h1 * k), REXP(e2 - h2 * k), &V);
 }
 
 /* compute_stress_from_F_trial, :467-526 */
-static void compute_stress(sim_t* s, int p, real dt) {
+static void compute_stress(sim_t* s, int p, real dt, probe_t* pr) {
     if (s->selection[p] != 0) return;
     const int mat = s->material[p];
     m3 Ft, F;
     memcpy(Ft.m, s->f[F_FTRIAL] + 9 * (size_t)p, sizeof(Ft.m));
-    if (mat == 1) F = return_von_mises(s, p, &Ft, 0);
-    else if (mat == 2) F = return_sand(s, p, &Ft);
-    else if (mat == 3) F = return_viscoplastic(s, p, &Ft, dt);
-    else if (mat == 5) F = return_von_mises(s, p, &Ft, 1);
+    if (mat == 1) F = return_von_mises(s, p, &Ft, 0, pr);
+    else if (mat == 2) F = return_sand(s, p, &Ft, pr);
+    else if (mat == 3) F = return_viscoplastic(s, p, &Ft, dt, pr);
+    else if (mat == 5) F = return_von_mises(s, p, &Ft, 1, pr);
     else F = Ft;
     memcpy(s->f[F_F] + 9 * (size_t)p, F.m, sizeof(F.m));
     const real J = m3_det(&F);
@@ -652,7 +672,17 @@ void mpmref_svd3(const double* F9, double* U9, double* sig3, double* V9) {
     for (int i = 0; i < 9; ++i) { U9[i] = U.m[i]; V9[i] = V.m[i]; }
     for (int i = 0; i < 3; ++i) sig3[i] = sg[i];
 }
-void mpmref_stress_of_F(sim_t* s, int p) { compute_stress(s, p, (real)1e-4); }
+void mpmref_stress_of_F(sim_t* s, int p) { compute_stress(s, p, (real)1e-4, NULL); }
+/* compute_stress of every particle (dt = 1e-4) with branch decisions inverted by `flip` (see probe_t); margins: [n][2]
+ * distances of the decisions from their boundaries, +inf where a decision was not reached */
+void mpmref_stress_probe(sim_t* s, int flip, double* margins) {
+    for (int p = 0; p < s->n; ++p) {
+        probe_t pr = {flip, {HUGE_VAL, HUGE_VAL}};
+        compute_stress(s, p, (real)1e-4, &pr);
+        margins[2 * p] = pr.margin[0];
+        margins[2 * p + 1] = pr.margin[1];
+    }
+}
 
 /* one p2g2p (mpm_solver_warp.py:514-637) */
 static void substep(sim_t* s, double dt_d) {
@@ -663,7 +693,7 @@ static void substep(sim_t* s, double dt_d) {
     memset(s->grid_m, 0, nodes * sizeof(real));
     memset(s->grid_v_in, 0, 3 * nodes * sizeof(real));
 #pragma omp parallel for schedule(static)
-    for (int p = 0; p < n; ++p) { particle_bcs(s, p, time, dt); compute_stress(s, p, dt); }
+    for (int p = 0; p < n; ++p) { particle_bcs(s, p, time, dt); compute_stress(s, p, dt, NULL); }
     if (s->parallel_p2g) {
 #pragma omp parallel for schedule(static)
         for (int p = 0; p < n; ++p) p2g_particle(s, p, dt);
@@ -691,7 +721,7 @@ void mpmref_set_active(sim_t* s, int n_active) { s->n = n_active; }
 void mpmref_scatter(sim_t* s, double dt_d) {
     const real dt = (real)dt_d;
     const float time = (float)s->time;
-    for (int p = 0; p < s->n; ++p) { particle_bcs(s, p, time, dt); compute_stress(s, p, dt); }
+    for (int p = 0; p < s->n; ++p) { particle_bcs(s, p, time, dt); compute_stress(s, p, dt, NULL); }
     for (int p = 0; p < s->n; ++p) p2g_particle(s, p, dt);
 }
 void mpmref_finish(sim_t* s, double dt_d, int x_begin, int x_end) {

@@ -55,6 +55,7 @@ def _lib(precision: str) -> C.CDLL:
     lib.mpmref_select_box.argtypes = [C.c_void_p, D, D, C.POINTER(C.c_int)]
     lib.mpmref_select_cylinder.argtypes = [C.c_void_p, D, D, C.c_double, C.c_double, C.POINTER(C.c_int)]
     lib.mpmref_stress_of_F.argtypes = [C.c_void_p, C.c_int]
+    lib.mpmref_stress_probe.argtypes = [C.c_void_p, C.c_int, D]
     lib.mpmref_step.argtypes = [C.c_void_p, C.c_int, C.c_double]
     lib.mpmref_num_threads.restype = C.c_int
     lib.mpmref_set_num_threads.argtypes = [C.c_int]
@@ -189,6 +190,14 @@ class MpmRef:
 
     def stress_of(self, p: int):
         self.lib.mpmref_stress_of_F(self.h, p)
+
+    def stress_probe(self, flip: int = 0) -> np.ndarray:
+        """`stress_of` for every particle, with the branch decisions whose bits are set in `flip` inverted (bit 0: the
+        plastic branch of a return map; bit 1: sand's cone-tip projection / the damage map's mu = lam = 0). Returns each
+        particle's two decision margins (relative distance from the boundary, > 0 = taken; inf = not reached)."""
+        out = np.zeros(2 * self.n)
+        self.lib.mpmref_stress_probe(self.h, int(flip), _dp(out))
+        return out.reshape(self.n, 2)
 
     def step(self, n_substeps: int, dt: float):
         self.lib.mpmref_step(self.h, int(n_substeps), float(dt))

@@ -170,6 +170,27 @@ class OracleBackend:
         return {"grid_m": m, "grid_v_in": vi, "grid_v_out": vo}
 
 
+class _DeviceArray:
+    """A device pointer presented through __cuda_array_interface__, so torch can copy from it."""
+
+    def __init__(self, ptr, shape, typestr="<f4"):
+        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (int(ptr), False), "version": 3,
+                                         "strides": None}
+
+
+def device_grid_v(s) -> np.ndarray:
+    """Grid velocities of the last substep, [n, n, n, 3], read through pixie_mpm_grid_ptrs. Only nodes inside the
+    particles' node box are swept; the solver leaves the others as they were."""
+    import ctypes as C
+    from pixie_b200 import _lib
+    mv, v = C.c_void_p(), C.c_void_p()
+    _lib.check(_lib.load().pixie_mpm_grid_ptrs(s._handle, C.byref(mv), C.byref(v)))
+    n = int(s.mpm_model.n_grid)
+    torch.cuda.synchronize()
+    g = torch.as_tensor(_DeviceArray(v.value, (n, n, n, 4)), device=s._device).clone()
+    return g[..., :3].cpu().numpy()
+
+
 class CudaBackend:
     """pixie_b200.mpm_solver_warp.MPM_Simulator_WARP on cuda:0 (every call goes through the C ABI)."""
     device = "cuda:0"
@@ -193,4 +214,4 @@ class CudaBackend:
         return [m.cpu().numpy() for m in s._masks]
 
     def get_grid(self, s):
-        return {}
+        return {"grid_v_out": device_grid_v(s)}
