@@ -3,6 +3,7 @@
 #include "ptx.cuh"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 
@@ -28,6 +29,11 @@ struct SmemCtrl {
 };
 
 constexpr int kCtlBarrierBytes = 512;     // SmemCtrl
+// channel-major epilogue: per consumer warpgroup, a staging chunk of kCmChunk voxels x 64 channels (rows padded to 68 floats:
+// the fragment writes hit 32 distinct banks, the 16-byte row reads stay aligned)
+constexpr int kCmChunk = 16;
+constexpr int kCmStageLd = 68;
+constexpr int kCmStageFloats = kCmChunk * kCmStageLd;
 constexpr int kStatsMaxC = 256;
 // statistics rows: [2][stats_ld] floats (sum, sum of squares) shared by the consumer warps (shared-memory atomics)
 
@@ -65,28 +71,28 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvKernelParams& p, int 
     return t;
 }
 
-// One (plane, kh) block: four K steps of 32 bytes (16 fp16 or 32 E5M2 values) over all BN columns, in chunks of at most 64
-// columns, as one wgmma group. Branch-free between fence and commit: ptxas serialises wgmma on any branch in between.
-template <int BN, bool F8>
+// One wgmma group: four K steps of 32 bytes (16 fp16 or 32 E5M2 values) of D[64 x N] += A[64 x K] * B[N x K]^T, both
+// operands K-major SW128 rows in shared memory. Voxel-major: A = slab rows (voxels), B = weight rows (N = block_n output
+// channels). Channel-major: A = weight rows (64 output channels), B = slab rows (N = the tile's voxels of one plane).
+// Branch-free between fence and commit: ptxas serialises wgmma on any branch in between.
+template <int N, bool F8>
 __device__ __forceinline__ void mma_block(float* acc, uint32_t a, uint32_t b) {
-    constexpr int NCH = BN < 64 ? BN : 64;
     wgmma_fence();
 #pragma unroll
     for (int k4 = 0; k4 < 4; ++k4) {
-        const uint64_t da = make_sw128_desc(a + 32u * k4);
-#pragma unroll
-        for (int s = 0; s < BN / NCH; ++s) {
-            const uint64_t db = make_sw128_desc(b + (uint32_t)(s * NCH * 128) + 32u * k4);
-            float* d = acc + s * NCH / 2;
-            if (F8) {
-                if (NCH == 16) wgmma_e5m2_n16(d, da, db);
-                if (NCH == 32) wgmma_e5m2_n32(d, da, db);
-                if (NCH == 64) wgmma_e5m2_n64(d, da, db);
-            } else {
-                if (NCH == 16) wgmma_f16_n16(d, da, db);
-                if (NCH == 32) wgmma_f16_n32(d, da, db);
-                if (NCH == 64) wgmma_f16_n64(d, da, db);
-            }
+        const uint64_t da = make_sw128_desc(a + 32u * k4), db = make_sw128_desc(b + 32u * k4);
+        if (F8) {
+            if (N == 16) wgmma_e5m2_n16(acc, da, db);
+            if (N == 32) wgmma_e5m2_n32(acc, da, db);
+            if (N == 64) wgmma_e5m2_n64(acc, da, db);
+            if (N == 128) wgmma_e5m2_n128(acc, da, db);
+            if (N == 256) wgmma_e5m2_n256(acc, da, db);
+        } else {
+            if (N == 16) wgmma_f16_n16(acc, da, db);
+            if (N == 32) wgmma_f16_n32(acc, da, db);
+            if (N == 64) wgmma_f16_n64(acc, da, db);
+            if (N == 128) wgmma_f16_n128(acc, da, db);
+            if (N == 256) wgmma_f16_n256(acc, da, db);
         }
     }
     wgmma_commit();
@@ -131,6 +137,46 @@ __device__ __forceinline__ int issue_slab(float (&acc)[TD][BN / 2], uint32_t a_a
     return groups;
 }
 
+// TMA producer loop (one warp; one elected lane issues): per tile and phase, the phase's weight tiles into a weight stage,
+// then the tde + n_kd - 1 input-plane slabs into the slab ring. Shared by both orientations, whose stages hold the same
+// rows (block_n weight rows per tap, TW x (TH + n_kh - 1) slab rows).
+__device__ __forceinline__ void produce_tiles(const ConvKernelParams& p, SmemCtrl* ctl, uint8_t* w_smem, uint8_t* s_smem,
+                                              volatile int* abort_flag, int total_items) {
+    int ws = 0, wph = 0, ss = 0, sph = 0;
+    bool ok = true;
+    for (int wi = blockIdx.x; wi < total_items && ok; wi += gridDim.x) {
+        const TileCoord t = decode_tile(p, wi);
+        for (int ph = t.ph_begin; ph < t.ph_end && ok; ++ph) {
+            const ConvPhase P = p.phases[ph];
+            const int ntaps = P.n_kh * P.n_kd;
+            ok = mbar_wait(&ctl->wempty[ws], wph ^ 1, abort_flag);
+            if (!ok) break;
+            if (elect_one()) {
+                mbar_expect_tx(&ctl->wfull[ws], (uint32_t)(ntaps * p.block_n * 128));
+                uint8_t* wdst = w_smem + (size_t)ws * p.w_stage_bytes;
+                for (int tap = 0; tap < ntaps; ++tap)
+                    tma_load_2d(wdst + (size_t)tap * p.block_n * 128, &p.tmB, &ctl->wfull[ws],
+                                (P.wtile_base + tap) * 64, t.n0);
+            }
+            if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
+
+            const int nplanes = t.tde + P.n_kd - 1;
+            const uint32_t slab_bytes = (uint32_t)p.slab_rows[P.src] * 128u;
+            for (int pl = 0; pl < nplanes && ok; ++pl) {
+                ok = mbar_wait(&ctl->sempty[ss], sph ^ 1, abort_flag);
+                if (!ok) break;
+                if (elect_one()) {
+                    mbar_expect_tx(&ctl->sfull[ss], slab_bytes);
+                    tma_load_5d(s_smem + (size_t)ss * p.s_stage_bytes, &p.tmA[P.src],
+                                &ctl->sfull[ss], (int)P.c0, t.w0 * p.stride + P.dw,
+                                t.h0 * p.stride + P.dh0, (t.d0 + pl) * p.stride + P.dd0, t.nb);
+                }
+                if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
+            }
+        }
+    }
+}
+
 }  // namespace
 
 template <int BN, int TD>
@@ -172,39 +218,7 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
 
     if (warp == kProducerWarp) {
         // ================================================================ TMA producer (warp-uniform, one elected lane issues)
-        int ws = 0, wph = 0, ss = 0, sph = 0;
-        bool ok = true;
-        for (int wi = blockIdx.x; wi < total_items && ok; wi += gridDim.x) {
-            const TileCoord t = decode_tile(p, wi);
-            for (int ph = t.ph_begin; ph < t.ph_end && ok; ++ph) {
-                const ConvPhase P = p.phases[ph];
-                const int ntaps = P.n_kh * P.n_kd;
-                ok = mbar_wait(&ctl->wempty[ws], wph ^ 1, abort_flag);
-                if (!ok) break;
-                if (elect_one()) {
-                    mbar_expect_tx(&ctl->wfull[ws], (uint32_t)(ntaps * p.block_n * 128));
-                    uint8_t* wdst = w_smem + (size_t)ws * p.w_stage_bytes;
-                    for (int tap = 0; tap < ntaps; ++tap)
-                        tma_load_2d(wdst + (size_t)tap * p.block_n * 128, &p.tmB, &ctl->wfull[ws],
-                                    (P.wtile_base + tap) * 64, t.n0);
-                }
-                if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
-
-                const int nplanes = t.tde + P.n_kd - 1;
-                const uint32_t slab_bytes = (uint32_t)p.slab_rows[P.src] * 128u;
-                for (int pl = 0; pl < nplanes && ok; ++pl) {
-                    ok = mbar_wait(&ctl->sempty[ss], sph ^ 1, abort_flag);
-                    if (!ok) break;
-                    if (elect_one()) {
-                        mbar_expect_tx(&ctl->sfull[ss], slab_bytes);
-                        tma_load_5d(s_smem + (size_t)ss * p.s_stage_bytes, &p.tmA[P.src],
-                                    &ctl->sfull[ss], (int)P.c0, t.w0 * p.stride + P.dw,
-                                    t.h0 * p.stride + P.dh0, (t.d0 + pl) * p.stride + P.dd0, t.nb);
-                    }
-                    if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
-                }
-            }
-        }
+        produce_tiles(p, ctl, w_smem, s_smem, abort_flag, total_items);
     } else {
         // ================================================================ consumers: MMA + epilogue (warpgroups 0 and 1)
         // Each warpgroup owns rows 64 g .. 64 g + 63 of the 128-voxel plane tile and the TD plane accumulators of those rows in
@@ -402,6 +416,221 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
     if (threadIdx.x == 0 && ctl->abort_flag && p.err_flag) atomicExch(p.err_flag, 1 + (int)blockIdx.x);
 }
 
+// Channel-major instance: D[co][vox] = W[co][k] * S[vox][k]^T. A tile is 64 output channels x NV voxels (TH x TW of one plane)
+// x 2 planes; consumer warpgroup g owns output plane d0 + g, so one wgmma is m64 nNV (n256 for 16 x 16 tiles) and a slab
+// still feeds both warpgroups through its kd taps. The weight rows of a phase are the A operand, the slab rows the B operand;
+// the phase table, slab ring and barriers are those of the voxel-major kernel. The accumulator is NV / 2 registers per
+// thread: the producer warpgroup hands its registers to the two consumer warpgroups (setmaxnreg).
+template <int NV>
+__global__ void __launch_bounds__(kConvCmThreads, 1)
+conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
+    constexpr int TW = NV == 64 ? 8 : 16;
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>(
+        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+    uint8_t* w_smem = smem;
+    uint8_t* s_smem = smem + (size_t)p.w_stages * p.w_stage_bytes;
+    SmemCtrl* ctl = reinterpret_cast<SmemCtrl*>(s_smem + (size_t)p.s_stages * p.s_stage_bytes);
+    float* stage_sm = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ctl) + kCtlBarrierBytes);   // epilogue staging
+    float* stats_sm = stage_sm + 2 * kCmStageFloats;                                                   // used iff p.stats
+    const int stats_ld = p.stats_ld;
+    const bool smem_misaligned = (p.smem_slack == 0) && (smem != smem_raw);
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int total_items = p.NB * p.tiles_d * p.tiles_h * p.tiles_w * p.n_tiles * p.split_k;
+    const bool do_stats = p.stats != nullptr;
+    const bool scalar_stats = do_stats && p.stats_scalar;
+
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < kMaxWStages; ++i) { mbar_init(&ctl->wfull[i], 1); mbar_init(&ctl->wempty[i], kConsumerWarps); }
+        for (int i = 0; i < kMaxSStages; ++i) { mbar_init(&ctl->sfull[i], 1); mbar_init(&ctl->sempty[i], kConsumerWarps); }
+        ctl->abort_flag = smem_misaligned ? 1 : 0;
+        fence_barrier_init();
+    }
+    if (warp == kProducerWarp && lane == 0) {
+        for (int i = 0; i < kConvMaxSrc; ++i) prefetch_tmap(&p.tmA[i]);
+        prefetch_tmap(&p.tmB);
+    }
+    if (do_stats && !scalar_stats)
+        for (int i = threadIdx.x; i < 2 * stats_ld; i += kConvCmThreads) stats_sm[i] = 0.f;
+    __syncthreads();
+    volatile int* abort_flag = &ctl->abort_flag;
+
+    if (warp >= kProducerWarp) {
+        // ================================================================ producer warpgroup: one warp issues the TMA loads
+        setmaxnreg_dec<40>();
+        if (warp == kProducerWarp) produce_tiles(p, ctl, w_smem, s_smem, abort_flag, total_items);
+    } else {
+        // ================================================================ consumers: warpgroup g computes plane d0 + g
+        setmaxnreg_inc<232>();
+        const int g = warp >> 2, wq = warp & 3, wt = threadIdx.x & 127;
+        float acc[NV / 2];
+        int ws = 0, wph = 0, ss = 0, sph = 0;
+        const uint32_t w_base0 = smem_u32(w_smem), s_base0 = smem_u32(s_smem);
+        bool ok = true;
+        const int ct = threadIdx.x;             // 0..255 among the consumer threads
+        int stats_nb = -1;
+        double tot_s = 0.0, tot_q = 0.0;
+        auto flush_stats = [&](int nb) {
+            if (scalar_stats) {
+#pragma unroll
+                for (int off = 16; off >= 1; off >>= 1) {
+                    tot_s += __shfl_xor_sync(0xffffffffu, tot_s, off);
+                    tot_q += __shfl_xor_sync(0xffffffffu, tot_q, off);
+                }
+                if (lane == 0) {
+                    atomicAdd(p.stats + (size_t)nb * p.Cout * 2, tot_s);
+                    atomicAdd(p.stats + (size_t)nb * p.Cout * 2 + 1, tot_q);
+                }
+                tot_s = 0.0; tot_q = 0.0;
+                return;
+            }
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            for (int ch = ct; ch < p.Cout; ch += 256) {
+                atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2, (double)stats_sm[ch]);
+                atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2 + 1, (double)stats_sm[stats_ld + ch]);
+                stats_sm[ch] = 0.f;
+                stats_sm[stats_ld + ch] = 0.f;
+            }
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+        };
+        // epilogue read-out: this thread's channel quad and voxel row inside a staged chunk
+        const int q4 = wt & 15, vr = wt >> 4;
+        float* stage = stage_sm + g * kCmStageFloats;
+
+        for (int wi = blockIdx.x; wi < total_items && ok; wi += gridDim.x) {
+            const TileCoord t = decode_tile(p, wi);
+#pragma unroll
+            for (int j = 0; j < NV / 2; ++j) acc[j] = 0.f;
+            const bool has_plane = g < t.tde;   // warpgroup-uniform
+            int pend_s = -1, pend_w = -1;
+            int prev_f8 = -1;
+            auto release = [&]() {
+                if (lane == 0) {
+                    if (pend_s >= 0) mbar_arrive(&ctl->sempty[pend_s]);
+                    if (pend_w >= 0) mbar_arrive(&ctl->wempty[pend_w]);
+                }
+                pend_s = -1; pend_w = -1;
+            };
+            for (int ph = t.ph_begin; ph < t.ph_end && ok; ++ph) {
+                const ConvPhase P = p.phases[ph];
+                const int n_kd = P.n_kd, n_kh = P.n_kh;
+                const bool f8 = P.f8 != 0;
+                if (prev_f8 >= 0 && prev_f8 != (int)f8) wgmma_wait<0>();
+                prev_f8 = (int)f8;
+                ok = mbar_wait(&ctl->wfull[ws], wph, abort_flag);
+                if (!ok) break;
+                const uint32_t w_addr = w_base0 + (uint32_t)(ws * p.w_stage_bytes);
+                const int nplanes = t.tde + n_kd - 1;
+                for (int pl = 0; pl < nplanes && ok; ++pl) {
+                    ok = mbar_wait(&ctl->sfull[ss], sph, abort_flag);
+                    if (!ok) break;
+                    const int kd = pl - g;
+                    int groups = 0;
+                    if (has_plane && kd >= 0 && kd < n_kd) {
+                        const uint32_t s_addr = s_base0 + (uint32_t)(ss * p.s_stage_bytes);
+                        for (int kh = 0; kh < n_kh; ++kh) {
+                            const uint32_t a = w_addr + (uint32_t)((kh * n_kd + (n_kd - 1 - kd)) * 64 * 128);
+                            const uint32_t b = s_addr + (uint32_t)(kh * TW * 128);
+                            if (f8) mma_block<NV, true>(acc, a, b);
+                            else mma_block<NV, false>(acc, a, b);
+                            ++groups;
+                        }
+                    }
+                    wgmma_wait_n(groups);          // the previous slab's MMAs have retired
+                    release();
+                    pend_s = ss;
+                    if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
+                }
+                pend_w = ws;
+                if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
+                if (p.w_stages == 1) { wgmma_wait<0>(); release(); }
+            }
+            wgmma_wait<0>();
+            release();
+#pragma unroll
+            for (int j = 0; j < NV / 2; ++j) fence_operand(acc[j]);
+            if (!ok) break;
+
+            // ---------------------------------------------------------------- epilogue through shared memory
+            // The fragment holds 2 channels x NV / 4 voxels per thread; it is staged in chunks of kCmChunk voxels x 64
+            // channels so that every output row is written (and the residual read) as 16-byte vectors.
+            if (do_stats && stats_nb != t.nb) {
+                if (stats_nb >= 0) flush_stats(stats_nb);
+                stats_nb = t.nb;
+            }
+            if (!has_plane) continue;
+            const bool first_split = (t.split == 0);
+            const int ch = t.n0 + 4 * q4;
+            const bool ch_ok = ch < p.Cout;      // Cout % 4 == 0 (plan)
+            float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (first_split && p.bias != nullptr && ch_ok)
+                bias4 = make_float4(__ldg(p.bias + ch), __ldg(p.bias + ch + 1), __ldg(p.bias + ch + 2), __ldg(p.bias + ch + 3));
+            const bool use_res = first_split && p.residual != nullptr;
+            const long long plane_base = ((long long)t.nb * p.D + t.d0 + g) * p.H;
+            float st_s[4] = {0.f, 0.f, 0.f, 0.f}, st_q[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+            for (int c = 0; c < NV / kCmChunk; ++c) {
+#pragma unroll
+                for (int jj = 0; jj < kCmChunk / 8; ++jj)
+#pragma unroll
+                    for (int r2 = 0; r2 < 2; ++r2)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int row = wq * 16 + (lane >> 2) + 8 * r2, v = jj * 8 + (lane & 3) * 2 + e;
+                            stage[v * kCmStageLd + row] = acc[(c * (kCmChunk / 8) + jj) * 4 + r2 * 2 + e];
+                        }
+                asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");
+#pragma unroll
+                for (int k = 0; k < kCmChunk / 8; ++k) {
+                    const int v = vr + 8 * k, vt = c * kCmChunk + v;
+                    const int hh = t.h0 + vt / TW, ww = t.w0 + vt % TW;
+                    float4 x = *reinterpret_cast<const float4*>(stage + v * kCmStageLd + 4 * q4);
+                    if (ch_ok && hh < p.H && ww < p.W) {
+                        const long long base = ((plane_base + hh) * p.W + ww) * p.out_ld + p.out_c0 + ch;
+                        x.x += bias4.x; x.y += bias4.y; x.z += bias4.z; x.w += bias4.w;
+                        if (use_res) {
+                            const float4 rv = __ldg(reinterpret_cast<const float4*>(p.residual + base));
+                            x.x += rv.x; x.y += rv.y; x.z += rv.z; x.w += rv.w;
+                        }
+                        if (p.atomic_out) red_add_v4(p.out + base, x.x, x.y, x.z, x.w);
+                        else *reinterpret_cast<float4*>(p.out + base) = x;
+                        st_s[0] += x.x; st_s[1] += x.y; st_s[2] += x.z; st_s[3] += x.w;
+                        st_q[0] = fmaf(x.x, x.x, st_q[0]); st_q[1] = fmaf(x.y, x.y, st_q[1]);
+                        st_q[2] = fmaf(x.z, x.z, st_q[2]); st_q[3] = fmaf(x.w, x.w, st_q[3]);
+                    }
+                }
+                asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");
+            }
+            if (do_stats) {
+                if (scalar_stats) {
+                    tot_s += (double)(st_s[0] + st_s[1] + st_s[2] + st_s[3]);
+                    tot_q += (double)(st_q[0] + st_q[1] + st_q[2] + st_q[3]);
+                } else {
+                    // lanes q4 and q4 + 16 of a warp hold the same channels: one shuffle, then shared atomics
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        st_s[i] += __shfl_xor_sync(0xffffffffu, st_s[i], 16);
+                        st_q[i] += __shfl_xor_sync(0xffffffffu, st_q[i], 16);
+                    }
+                    if (lane < 16 && ch_ok) {
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            atomicAdd(stats_sm + ch + i, st_s[i]);
+                            atomicAdd(stats_sm + stats_ld + ch + i, st_q[i]);
+                        }
+                    }
+                }
+            }
+        }
+        if (do_stats && stats_nb >= 0 && ok) flush_stats(stats_nb);
+    }
+
+    __syncthreads();
+    if (threadIdx.x == 0 && ctl->abort_flag && p.err_flag) atomicExch(p.err_flag, 1 + (int)blockIdx.x);
+}
+
 // =====================================================================================  host side
 
 int conv_k_total(const ConvDesc& d) {
@@ -536,7 +765,7 @@ void conv_pack_weights(const ConvDesc& d, const std::vector<const float*>& seg_w
     }
 }
 
-// Kernel instance for (block_n, TD); the plan guarantees a power-of-two block_n in 16..128, TD in {1, 2, 4}, TD * block_n <= 128.
+// Voxel-major instance for (block_n, TD); the plan guarantees block_n in {16, 32}, TD in {1, 2, 4}.
 static ConvKernelFn conv_kernel_for(int bn, int td) {
     switch (bn * 8 + td) {
         case 16 * 8 + 1: return conv3d_igemm_kernel<16, 1>;
@@ -544,10 +773,16 @@ static ConvKernelFn conv_kernel_for(int bn, int td) {
         case 16 * 8 + 4: return conv3d_igemm_kernel<16, 4>;
         case 32 * 8 + 1: return conv3d_igemm_kernel<32, 1>;
         case 32 * 8 + 2: return conv3d_igemm_kernel<32, 2>;
-        case 32 * 8 + 4: return conv3d_igemm_kernel<32, 4>;
-        case 64 * 8 + 1: return conv3d_igemm_kernel<64, 1>;
-        case 64 * 8 + 2: return conv3d_igemm_kernel<64, 2>;
-        default: return conv3d_igemm_kernel<128, 1>;
+        default: return conv3d_igemm_kernel<32, 4>;
+    }
+}
+
+// Channel-major instance for NV voxels per plane tile (64, 128 or 256).
+static ConvKernelFn conv_cm_kernel_for(int nv) {
+    switch (nv) {
+        case 64: return conv3d_igemm_cm_kernel<64>;
+        case 128: return conv3d_igemm_cm_kernel<128>;
+        default: return conv3d_igemm_cm_kernel<256>;
     }
 }
 
@@ -606,9 +841,8 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     ConvKernelParams& p = plan.p;
     memset(&p, 0, sizeof(p));
     p.NB = d.NB; p.D = d.D; p.H = d.H; p.W = d.W; p.stride = d.stride;
-    p.TW = (d.W >= 16) ? 16 : 8;
-    p.TH = 128 / p.TW;
     p.Cout = d.Cout;
+    const int out_ld = d.out_ld ? d.out_ld : d.Cout;
 
     const auto slots = conv_src_slots(d);
     if ((int)slots.size() > kConvMaxSrc) return fail("too many (source, tap-class) slots");
@@ -622,34 +856,66 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 
-    // N tile: a power of two (16 .. 128); columns past Cout_pad are zero-filled by the weight TMA and never stored
-    int bn = d.block_n;
-    if (bn == 0) {
-        bn = 16;
-        while (bn < std::min(any3 ? 64 : 128, d.Cout_pad)) bn *= 2;
+    // Orientation. Channel-major puts 64 output channels on the wgmma M side and up to 256 voxels on N: the widest MMA, the
+    // least shared-memory operand traffic per MAC and a phase's weights reused over up to 512 voxels. It needs outputs of at
+    // least 64 channels (M is 64 wide) written as 16-byte NDHWC vectors; the narrow heads and the projector, which would
+    // leave most of M empty, and planar outputs take the voxel-major kernel.
+    plan.channel_major = d.Cout >= 64 && d.Cout % 4 == 0 && !d.out_planar && out_ld % 4 == 0 && d.out_c0 % 4 == 0 &&
+                         reinterpret_cast<uintptr_t>(d.out) % 16 == 0 && reinterpret_cast<uintptr_t>(d.residual) % 16 == 0;
+    int bn = 0, td = 0, nv = 0;
+    if (plan.channel_major) {
+        bn = 64;
+        td = 2;
+        // voxel tile: 16 x 16, 8 x 16 or 8 x 8 of one plane. Wave quantisation: a persistent grid of `sms` CTAs finishes in
+        // ceil(tiles/sms) rounds; prefer the tile with the best last-round fill times the share of real voxels, each halving
+        // of NV costing ~7 % (more weight and slab traffic per MAC, narrower MMAs)
+        auto score = [&](int v, double& best) {
+            const int tw = v == 64 ? 8 : 16, th = v / tw;
+            const long long tx = (d.W + tw - 1) / tw, ty = (d.H + th - 1) / th;
+            const long long tiles = (long long)d.NB * tx * ty * ((d.D + 1) / 2) * ((d.Cout_pad + 63) / 64);
+            const long long rounds = (tiles + sms - 1) / sms;
+            const double sc = (double)tiles / (double)(rounds * sms) * (double)d.W * d.H / (double)(tx * tw * ty * th) *
+                              std::pow(0.93, v == 256 ? 0 : v == 128 ? 1 : 2);
+            if (sc > best) { best = sc; nv = v; }
+        };
+        if (d.nv) {
+            if (d.nv != 64 && d.nv != 128 && d.nv != 256) return fail("bad nv");
+            nv = d.nv;
+        } else {
+            double best = -1.0;
+            for (int v : {256, 128, 64})
+                if (v == 64 || d.W >= 16) score(v, best);
+        }
+        p.TW = nv == 64 ? 8 : 16;
+        p.TH = nv / p.TW;
+    } else {
+        p.TW = (d.W >= 16) ? 16 : 8;
+        p.TH = 128 / p.TW;
+        // N tile: 16 or 32; columns past Cout_pad are zero-filled by the weight TMA and never stored
+        bn = d.block_n;
+        if (bn == 0) bn = d.Cout_pad > 16 ? 32 : 16;
+        if (bn != 16 && bn != 32) return fail("bad block_n");
+
+        // TD: output planes per tile. Their accumulators live in the consumer warpgroups' registers: TD * block_n <= 128
+        // fp32 columns (64 registers per thread).
+        td = d.td ? d.td : std::min(4, 128 / bn);
+        td = std::max(1, std::min(td, d.D));
+        if (!any3 && !d.td) td = std::min(td, 2);    // no plane re-use without kd taps: smaller tiles, more CTAs (unless forced)
+        if (td == 3) td = 2;                // the kernel is instantiated for TD = 1, 2, 4
+        if (td * bn > 128) return fail("TD*block_n exceeds the register accumulator budget (128)");
+        if (!d.td && td > 1) {
+            // wave quantisation: prefer the plane count with the better last-round fill
+            auto fill = [&](int t) {
+                const long long tiles = (long long)d.NB * ((d.W + p.TW - 1) / p.TW) * ((d.H + p.TH - 1) / p.TH) * ((d.D + t - 1) / t) *
+                                        ((d.Cout_pad + bn - 1) / bn);
+                const long long rounds = (tiles + sms - 1) / sms;
+                return (double)tiles / (double)(rounds * sms) * (t == td ? 1.0 : 0.93);   // halving TD costs ~7 % more slab traffic
+            };
+            if (fill(td / 2) > fill(td)) td /= 2;
+        }
     }
-    if (bn != 16 && bn != 32 && bn != 64 && bn != 128) return fail("bad block_n");
     p.block_n = bn;
     p.n_tiles = (d.Cout_pad + bn - 1) / bn;
-
-    // TD: output planes per tile. Their accumulators live in the consumer warpgroups' registers: TD * block_n <= 128
-    // fp32 columns (64 registers per thread; registers are allocated per warpgroup, so 288 threads get at most 168 each).
-    int td = d.td ? d.td : std::min(4, 128 / bn);
-    td = std::max(1, std::min(td, d.D));
-    if (!any3 && !d.td) td = std::min(td, 2);    // no plane re-use without kd taps: smaller tiles, more CTAs (unless forced)
-    if (td == 3) td = 2;                // the kernel is instantiated for TD = 1, 2, 4
-    if (td * bn > 128) return fail("TD*block_n exceeds the register accumulator budget (128)");
-    if (!d.td && td > 1) {
-        // wave quantisation: a persistent grid of `sms` CTAs finishes in ceil(tiles/sms) rounds; prefer the
-        // plane count with the better last-round fill
-        auto fill = [&](int t) {
-            const long long tiles = (long long)d.NB * ((d.W + p.TW - 1) / p.TW) * ((d.H + p.TH - 1) / p.TH) * ((d.D + t - 1) / t) *
-                                    ((d.Cout_pad + bn - 1) / bn);
-            const long long rounds = (tiles + sms - 1) / sms;
-            return (double)tiles / (double)(rounds * sms) * (t == td ? 1.0 : 0.93);   // halving TD costs ~7 % more slab traffic
-        };
-        if (fill(td / 2) > fill(td)) td /= 2;
-    }
     p.TD = td;
     p.tiles_w = (d.W + p.TW - 1) / p.TW;
     p.tiles_h = (d.H + p.TH - 1) / p.TH;
@@ -679,7 +945,7 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     plan.fused_stats = d.stats != nullptr && split == 1 && d.Cout <= kStatsMaxC && !d.out_planar;
     p.stats_ld = (d.Cout + 31) / 32 * 32;
     const int stats_bytes = plan.fused_stats ? 2 * p.stats_ld * 4 : 0;
-    const int ctl_core = kCtlBarrierBytes + stats_bytes;
+    const int ctl_core = kCtlBarrierBytes + (plan.channel_major ? 2 * kCmStageFloats * 4 : 0) + stats_bytes;
     auto plan_stages = [&](int slack, int& ws, int& ss) {
         const int avail = 227 * 1024 - ctl_core - slack;
         ws = (2 * p.w_stage_bytes + 2 * p.s_stage_bytes <= avail) ? 2 : 1;
@@ -713,7 +979,7 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     p.phases = plan.d_phases;
 
     p.bias = d.bias; p.residual = d.residual; p.out = d.out;
-    p.out_ld = d.out_ld ? d.out_ld : d.Cout; p.out_c0 = d.out_c0; p.out_planar = d.out_planar;
+    p.out_ld = out_ld; p.out_c0 = d.out_c0; p.out_planar = d.out_planar;
     p.err_flag = d_err_flag;
     p.stats = plan.fused_stats ? d.stats : nullptr;
     p.stats_scalar = d.stats_scalar ? 1 : 0;
@@ -722,7 +988,8 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
 
     plan.grid = std::min(items * split, sms);
 
-    plan.kernel = conv_kernel_for(bn, td);
+    plan.kernel = plan.channel_major ? conv_cm_kernel_for(nv) : conv_kernel_for(bn, td);
+    plan.threads = plan.channel_major ? kConvCmThreads : kConvThreads;
     if (cudaFuncSetAttribute(plan.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
         return fail("cudaFuncSetAttribute(max dynamic smem)");
     return 0;
@@ -741,7 +1008,7 @@ int conv_plan_launch(const ConvPlan& plan, cudaStream_t stream) {
         // p.NB items, and clearing the planned count would write past its end.
         cudaMemsetAsync(plan.p.out, 0, plan.out_item_bytes * (size_t)plan.p.NB, stream);
     }
-    plan.kernel<<<plan.grid, kConvThreads, plan.smem_bytes, stream>>>(plan.p);
+    plan.kernel<<<plan.grid, plan.threads, plan.smem_bytes, stream>>>(plan.p);
     return (int)cudaGetLastError();
 }
 

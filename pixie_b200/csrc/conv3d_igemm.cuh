@@ -8,10 +8,14 @@
 // weights are packed per "phase" (see below) as fp16 [Cout_pad][K] with K contiguous, accumulation
 // is fp32 in registers, outputs are fp32 (NDHWC, or NCDHW planar for the network head).
 //
-// GEMM view: M = output voxels (tile = TD planes x TH x TW, TH*TW = 128 rows per accumulator),
-// N = output channels (BLOCK_N <= 128 per CTA tile), K = taps x input channels in chunks of 64.
-// Each of the two consumer warpgroups computes 64 of the 128 rows for all TD planes (TD * BLOCK_N <= 128 accumulator
-// columns, 64 fp32 registers per thread) and writes them out itself; one producer warp issues the TMA loads.
+// GEMM view, two orientations chosen by the planner from the output shape:
+//  * channel-major (every output of 64 or more channels): M = 64 output channels, N = NV voxels of one d-plane (TH x TW =
+//    8 x 8, 8 x 16 or 16 x 16), K = taps x input channels in chunks of 64. The two consumer warpgroups take the two planes of
+//    a TD = 2 tile (NV / 2 fp32 accumulator registers per thread) and write their outputs through shared memory; a producer
+//    warpgroup issues the TMA loads and hands its registers to them.
+//  * voxel-major (narrow outputs: the network heads, the 32-channel projector; planar outputs): M = output voxels (tile = TD planes x TH x
+//    TW, TH*TW = 128 rows per accumulator), N = output channels (BLOCK_N of 16 or 32 per CTA tile). Each of the two consumer
+//    warpgroups computes 64 of the 128 rows for all TD planes and writes them out itself; one producer warp issues the TMA loads.
 //
 // The K loop is organised in PHASES so that shared memory, not L2, serves the tap re-use:
 //   phase = (source tensor, 64-channel chunk, kw)  for 3x3x3 stride-1 convolutions.
@@ -33,7 +37,8 @@ namespace pixie {
 
 constexpr int kConvMaxSrc = 8;
 constexpr int kF8Shift = 6;        // power-of-two rebalancing between the E5M2 operands (see ConvDesc::Seg)
-constexpr int kConvThreads = 288;  // warps 0-7: two MMA + epilogue warpgroups, warp 8: TMA producer
+constexpr int kConvThreads = 288;    // voxel-major: warps 0-7: two MMA + epilogue warpgroups, warp 8: TMA producer
+constexpr int kConvCmThreads = 384;  // channel-major: warps 0-7 as above, warps 8-11: producer warpgroup (warp 8 issues)
 
 struct ConvPhase {        // 16 bytes, lives in global memory
     int8_t src;           // tensor-map index of the activation source
@@ -57,10 +62,10 @@ struct ConvKernelParams {
     // output geometry
     int NB, D, H, W;      // batch and OUTPUT spatial size
     int stride;           // 1 or 2
-    int TW, TH, TD;       // tile: TH*TW == 128, TD in {1, 2, 4}
+    int TW, TH, TD;       // tile: TH*TW == 128, TD in {1, 2, 4} (voxel-major); TH*TW == NV, TD == 2 (channel-major)
     int tiles_w, tiles_h, tiles_d;
     int Cout;             // real output channels
-    int block_n;          // N tile (power of two, 16 .. 128)
+    int block_n;          // output channels per tile: 16 or 32 (voxel-major), 64 (channel-major)
     int n_tiles;          // ceil(Cout / block_n)
     // shared-memory plan
     int w_stage_bytes, w_stages;   // weight stages (all taps of one phase)
@@ -117,8 +122,9 @@ struct ConvDesc {
     double* stats = nullptr;           // request fused output statistics (honoured iff plan.fused_stats)
     bool stats_scalar = false;         // totals only (see ConvKernelParams::stats_scalar)
     int split_k = 1;                   // >1 => atomics into pre-zeroed out
-    int block_n = 0;                   // 0 = choose; else 16, 32, 64 or 128
-    int td = 0;                        // 0 = choose
+    int block_n = 0;                   // voxel-major: 0 = choose; else 16 or 32
+    int td = 0;                        // voxel-major: 0 = choose
+    int nv = 0;                        // channel-major voxels per plane tile: 0 = choose; else 64, 128 or 256
 };
 
 // K_total (in elements) of a ConvDesc: sum over segments of ks^3 * C.
@@ -136,7 +142,9 @@ void conv_pack_weights(const ConvDesc& d, const std::vector<const float*>& seg_w
 struct ConvPlan {
     ConvKernelParams p{};
     ConvPhase* d_phases = nullptr;
-    ConvKernelFn kernel = nullptr;     // instance for (block_n, TD)
+    ConvKernelFn kernel = nullptr;     // instance for (block_n, TD) or, channel-major, NV
+    bool channel_major = false;
+    int threads = 0;                   // kConvThreads or kConvCmThreads
     int grid = 0;
     int smem_bytes = 0;
     bool needs_zero = false;   // out must be zeroed before launch (atomic_out)

@@ -51,7 +51,8 @@ struct Case {
     int Cout = 64;
     bool bias = true, residual = false, planar = false;
     int split_k = 1, block_n = 0, td = 0;  // 0: the planner chooses
-    bool forced = false;                   // block_n and td are forced: the plan must use exactly them
+    int nv = 0;                            // channel-major voxel tile; 0: the planner chooses
+    bool forced = false;                   // block_n and td (voxel-major) or nv (channel-major) are forced: the plan must use them
     bool want_split = false;               // the planner must choose split-K
     bool timing = false;
     int prec = kF16;
@@ -64,7 +65,7 @@ struct Totals {
     double r = 0, rx3 = 0, r8 = 0;         // max err/S (fp16 cases, fp16x3 cases), max (err - kTau S)/S8 (E5M2 cases)
     std::string r_case, rx3_case, r8_case;
     double e5_ratio = 1e30, x3_ratio = 1e30;   // min over cases of (single fp16 pass error) / (corrected error), vs a*w
-    std::map<std::pair<int, int>, int> inst;   // (block_n, TD) -> cases that ran on that kernel instance
+    std::map<std::string, int> inst;           // kernel instance ("vm(block_n,TD)" or "cm(NV)") -> cases that ran on it
     std::map<std::string, int> tags;
 };
 
@@ -86,7 +87,7 @@ static bool run_case(const Case& c, int* d_err, Totals& T) {
     ConvDesc d;
     d.NB = NB; d.D = d.H = d.W = Do; d.stride = c.stride; d.Cout = c.Cout;
     d.Cout_pad = (c.Cout + 15) / 16 * 16;
-    d.split_k = c.split_k; d.block_n = c.block_n; d.td = c.td; d.out_planar = c.planar;
+    d.split_k = c.split_k; d.block_n = c.block_n; d.td = c.td; d.nv = c.nv; d.out_planar = c.planar;
 
     // ---- activations, built the way the executor's normalise kernel stores them. Host copies are the decoded operands:
     // Ah = fp16(a), Al = fp16(a - Ah) (fp16x3), A1 = e5m2((a - Ah) 2^s), A2 = e5m2(a 2^-s) (fp16e5), At = a.
@@ -192,13 +193,17 @@ static bool run_case(const Case& c, int* d_err, Totals& T) {
         const int items = nl * pl.p.tiles_d * pl.p.tiles_h * pl.p.tiles_w * pl.p.n_tiles * pl.p.split_k;
         pl.grid = std::min(items, pl.grid);
     }
-    printf("[%s] %s NB=%d launched=%d grid=%d smem=%d bn=%d TD=%d TW=%d TH=%d w_stages=%d s_stages=%d phases=%d split=%d stats=%s%s\n",
-           c.name.c_str(), kPrecName[c.prec], NB, nl, pl.grid, pl.smem_bytes, pl.p.block_n, pl.p.TD, pl.p.TW, pl.p.TH,
+    const std::string inst = pl.channel_major ? "cm(" + std::to_string(pl.p.TH * pl.p.TW) + ")"
+                                              : "vm(" + std::to_string(pl.p.block_n) + "," + std::to_string(pl.p.TD) + ")";
+    printf("[%s] %s NB=%d launched=%d grid=%d smem=%d %s bn=%d TD=%d TW=%d TH=%d w_stages=%d s_stages=%d phases=%d split=%d stats=%s%s\n",
+           c.name.c_str(), kPrecName[c.prec], NB, nl, pl.grid, pl.smem_bytes, inst.c_str(), pl.p.block_n, pl.p.TD, pl.p.TW, pl.p.TH,
            pl.p.w_stages, pl.p.s_stages, pl.p.n_phases, pl.p.split_k, kStatsName[c.stats], plan.fused_stats ? " (fused)" : "");
     fflush(stdout);
     bool plan_ok = true;
-    if (c.forced && (pl.p.block_n != c.block_n || pl.p.TD != c.td)) {
-        printf("[%s] forced bn=%d TD=%d but the plan uses bn=%d TD=%d\n", c.name.c_str(), c.block_n, c.td, pl.p.block_n, pl.p.TD);
+    const std::string want = c.nv ? "cm(" + std::to_string(c.nv) + ")"
+                                  : "vm(" + std::to_string(c.block_n) + "," + std::to_string(c.td) + ")";
+    if (c.forced && inst != want) {
+        printf("[%s] forced %s but the plan uses %s\n", c.name.c_str(), want.c_str(), inst.c_str());
         plan_ok = false;
     }
     if (c.want_split && pl.p.split_k == 1) { printf("[%s] expected a split-K plan\n", c.name.c_str()); plan_ok = false; }
@@ -214,7 +219,7 @@ static bool run_case(const Case& c, int* d_err, Totals& T) {
         cleanup();
         return false;
     }
-    T.inst[{pl.p.block_n, pl.p.TD}]++;
+    T.inst[inst]++;
 
     if (c.timing) {
         cudaEvent_t e0, e1;
@@ -451,18 +456,35 @@ int main(int argc, char** argv) {
     add("x3", "x3_head_64_3_planar_d16_splitk", 2, 16, 1, 64, 3, 3, kX3).planar = true;
     cases.back().split_k = 0; cases.back().want_split = true;
 
-    // ---- every kernel instance, forced, on a 3x3x3 stride-1, a stride-2 and a 1x1 conv, in fp16 and with E5M2
+    // ---- every voxel-major kernel instance, forced, on a 3x3x3 stride-1, a stride-2 and a 1x1 conv with 48 output channels
+    // (a partial channel tile), in fp16 and with E5M2
+    const struct { const char* kind; int stride, ks, Cin; } kinds[] = {{"c3", 1, 3, 64}, {"s2", 2, 3, 64}, {"1x1", 1, 1, 128}};
     for (int prec : {kF16, kE5})
-        for (int bn : {16, 32, 64, 128})
+        for (int bn : {16, 32})
             for (int td : {1, 2, 4}) {
-                if (bn * td > 128) continue;
                 const std::string sfx = "_bn" + std::to_string(bn) + "_td" + std::to_string(td) + (prec == kE5 ? "_e5" : "");
-                const struct { const char* kind; int stride, ks, Cin; } kinds[] = {{"c3", 1, 3, 64}, {"s2", 2, 3, 64}, {"1x1", 1, 1, 128}};
                 for (const auto& k : kinds) {
-                    Case& c = add("instance", std::string("inst_") + k.kind + sfx, 1, 8, k.stride, k.Cin, k.ks, 96, prec);
+                    Case& c = add("instance", std::string("inst_") + k.kind + sfx, 1, 8, k.stride, k.Cin, k.ks, 48, prec);
                     c.block_n = bn; c.td = td; c.forced = true;
                 }
             }
+    // ---- every channel-major instance, forced: the same three kinds with 96 output channels (a partial channel tile) in
+    // fp16 and with E5M2, then at 9^3 (ragged sides for every tile, a last tile with one plane): concatenated sources with the
+    // fused skip and a residual, split-K, a short batch, each statistics mode
+    for (int nv : {64, 128, 256}) {
+        const std::string sn = "_nv" + std::to_string(nv);
+        auto force = [&](Case& c) { c.nv = nv; c.forced = true; return &c; };
+        for (int prec : {kF16, kE5})
+            for (const auto& k : kinds)
+                force(add("instance", std::string("cm_") + k.kind + sn + (prec == kE5 ? "_e5" : ""), 1, 8, k.stride, k.Cin, k.ks, 96, prec));
+        force(add_cat("instance", "cm_cat_skip_res_d9" + sn, 2, 9, 64, 128, 64, kE5))->residual = true;
+        { Case* c = force(add("instance", "cm_splitk_res_d9" + sn, 1, 9, 1, 128, 3, 128, kE5)); c->split_k = 3; c->residual = true;
+          c->want_split = true; }
+        { Case* c = force(add("instance", "cm_short_d9" + sn + "_nb3_launch2", 3, 9, 1, 64, 3, 64)); c->launch_nb = 2; c->residual = true; }
+        force(add("instance", "cm_scalar_stats_d9" + sn, 2, 9, 1, 64, 3, 64, kE5))->stats = kScalarStats;
+        force(add("instance", "cm_no_stats_s2_d9" + sn, 1, 9, 2, 64, 3, 64))->stats = kNoStats;
+        force(add("instance", "cm_x3_1x1_d9" + sn, 2, 9, 1, 128, 1, 64, kX3));
+    }
 
     // ---- ragged geometry: the grid sides the U-Net reaches at grid_size 24 / 48, partial depth and channel tiles
     for (int D : {3, 6, 12, 24}) add("ragged", "r_conv3_64_64_d" + std::to_string(D), D <= 6 ? 2 : 1, D, 1, 64, 3, 64);
@@ -474,7 +496,7 @@ int main(int argc, char** argv) {
     { Case& c = add("ragged", "r_td4_d6_tde2_e5", 1, 6, 1, 64, 3, 32, kE5); c.block_n = 32; c.td = 4; c.forced = true; }
     add("ragged", "r_cout8_d12", 1, 12, 1, 64, 3, 8);
     add("ragged", "r_cout80_d12", 1, 12, 1, 64, 3, 80).residual = true;
-    { Case& c = add("ragged", "r_cout192_bn128_d6", 2, 6, 1, 128, 3, 192); c.block_n = 128; c.td = 1; c.forced = true; }
+    add("ragged", "r_cout192_d6", 2, 6, 1, 128, 3, 192);
     add("ragged", "r_cout80_d6_e5", 1, 6, 1, 64, 3, 80, kE5);
     add_cat("ragged", "r_block_e5_cat_skip_128_64_d12", 2, 12, 64, 128, 64, kE5);          // 4 slots, fused statistics
     { Case& c = add("ragged", "r_head_e5_planar_splitk_d16", 2, 16, 1, 64, 3, 3, kE5); c.planar = true; c.split_k = 0; c.want_split = true; }
@@ -497,19 +519,18 @@ int main(int argc, char** argv) {
     add("stats", "st_none_x3_conv3_d6", 2, 6, 1, 64, 3, 64, kX3).stats = kNoStats;
 
     // ---- 64^3: several tiles per CTA and batch-item boundaries crossed (tile-edge sample), timed
-    auto add_t = [&](const std::string& name, int NB, int Cin, int ks, int Cout, int prec, int bn = 0, int td = 0) {
+    auto add_t = [&](const std::string& name, int NB, int Cin, int ks, int Cout, int prec) {
         Case& c = add("timing", name, NB, 64, 1, Cin, ks, Cout, prec);
-        c.timing = true; c.block_n = bn; c.td = td;
+        c.timing = true;
         return &c;
     };
     add_t("T_x2_conv3_64_64_d64_nb2", 2, 64, 3, 64, kE5);
     add_t("T_x2_conv3_128_64_d64", 1, 128, 3, 64, kE5)->residual = true;
     add_t("T_x3_conv3_64_64_d64", 1, 64, 3, 64, kX3);
+    add_t("T_x2_conv3_128_128_d64", 1, 128, 3, 128, kE5);
     add_t("T_conv3_64_64_d64", 1, 64, 3, 64, kF16);
-    add_t("T_conv3_64_64_d64_td2", 1, 64, 3, 64, kF16, 0, 2);
     add_t("T_conv3_128_64_d64", 1, 128, 3, 64, kF16)->residual = true;
     add_t("T_conv3_128_128_d64", 1, 128, 3, 128, kF16);
-    add_t("T_conv3_128_128_d64_bn128", 1, 128, 3, 128, kF16, 128);
     add_t("T_gemm1x1_512_128_d64", 1, 512, 1, 128, kF16);
     {
         Case& c = add("timing", "T_conv3_64_64_d32", 1, 32, 1, 64, 3, 64); c.timing = true;
@@ -527,16 +548,19 @@ int main(int argc, char** argv) {
         if (!run_case(c, d_err, T)) ++T.n_fail;
     }
 
-    printf("INSTANCES (block_n, TD): cases");
+    // every instance the planner can select: voxel-major (block_n, TD) and channel-major NV
+    printf("INSTANCES: cases");
     int missing = 0;
-    for (int bn : {16, 32, 64, 128})
-        for (int td : {1, 2, 4}) {
-            if (bn * td > 128) continue;
-            const auto it = T.inst.find({bn, td});
-            const int n = it == T.inst.end() ? 0 : it->second;
-            printf("  (%d,%d): %d", bn, td, n);
-            missing += n == 0;
-        }
+    std::vector<std::string> all;
+    for (int bn : {16, 32})
+        for (int td : {1, 2, 4}) all.push_back("vm(" + std::to_string(bn) + "," + std::to_string(td) + ")");
+    for (int nv : {64, 128, 256}) all.push_back("cm(" + std::to_string(nv) + ")");
+    for (const auto& k : all) {
+        const auto it = T.inst.find(k);
+        const int n = it == T.inst.end() ? 0 : it->second;
+        printf("  %s: %d", k.c_str(), n);
+        missing += n == 0;
+    }
     printf("\n");
     if (!filter[0] && missing) { printf("FAIL: %d kernel instance(s) not run\n", missing); ++T.n_fail; }
     printf("CASES by kind:");
