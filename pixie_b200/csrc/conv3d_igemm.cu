@@ -15,7 +15,7 @@ using namespace ptx;
 
 namespace {
 
-constexpr int kMaxWStages = 2;
+constexpr int kMaxWStages = 4;          // voxel-major: up to 2 phase stages; channel-major: up to 4 kd units
 constexpr int kMaxSStages = 8;
 constexpr int kConsumerWarps = 8;          // two warpgroups, 64 accumulator rows each
 constexpr int kProducerWarp = 8;
@@ -170,6 +170,51 @@ __device__ __forceinline__ void produce_tiles(const ConvKernelParams& p, SmemCtr
                     tma_load_5d(s_smem + (size_t)ss * p.s_stage_bytes, &p.tmA[P.src],
                                 &ctl->sfull[ss], (int)P.c0, t.w0 * p.stride + P.dw,
                                 t.h0 * p.stride + P.dh0, (t.d0 + pl) * p.stride + P.dd0, t.nb);
+                }
+                if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
+            }
+        }
+    }
+}
+
+// Channel-major producer: the weight ring holds one kd tap of a phase per stage (its n_kh tiles, 24 KB for a 3x3x3 phase), loaded
+// just ahead of the first slab that uses it: unit kd before slab kd. A unit is released as soon as its last slab retires instead of
+// at the end of the phase, so three units take the place of two whole-phase stages and the freed 72 KB buy two more slab stages.
+__device__ __forceinline__ void produce_tiles_cm(const ConvKernelParams& p, SmemCtrl* ctl, uint8_t* w_smem, uint8_t* s_smem,
+                                                 volatile int* abort_flag, int total_items) {
+    int ws = 0, wph = 0, ss = 0, sph = 0;
+    bool ok = true;
+    for (int wi = blockIdx.x; wi < total_items && ok; wi += gridDim.x) {
+        const TileCoord t = decode_tile(p, wi);
+        for (int ph = t.ph_begin; ph < t.ph_end && ok; ++ph) {
+            const ConvPhase P = p.phases[ph];
+            const int n_kd = P.n_kd, n_kh = P.n_kh, nplanes = t.tde + n_kd - 1;
+            const uint32_t slab_bytes = (uint32_t)p.slab_rows[P.src] * 128u, unit_bytes = (uint32_t)(n_kh * p.block_n * 128);
+            const CUtensorMap* tm = &p.tmA[P.src];
+            const int cw = t.w0 * p.stride + P.dw, ch = t.h0 * p.stride + P.dh0, cd = t.d0 * p.stride + P.dd0;
+            // packed tile order inside a phase: kh major, then kd = n_kd - 1 .. 0; unit kd starts at tile n_kd - 1 - kd
+            int wcol = (P.wtile_base + n_kd - 1) * 64;
+#pragma unroll 1
+            for (int pl = 0; pl < nplanes && ok; ++pl) {
+                if (pl < n_kd) {
+                    ok = mbar_wait(&ctl->wempty[ws], wph ^ 1, abort_flag);
+                    if (!ok) break;
+                    if (elect_one()) {
+                        mbar_expect_tx(&ctl->wfull[ws], unit_bytes);
+                        uint8_t* wdst = w_smem + (size_t)ws * p.w_stage_bytes;
+#pragma unroll 1
+                        for (int kh = 0; kh < n_kh; ++kh)
+                            tma_load_2d(wdst + (size_t)kh * p.block_n * 128, &p.tmB, &ctl->wfull[ws], wcol + kh * n_kd * 64, t.n0);
+                    }
+                    wcol -= 64;
+                    if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
+                }
+                ok = mbar_wait(&ctl->sempty[ss], sph ^ 1, abort_flag);
+                if (!ok) break;
+                if (elect_one()) {
+                    mbar_expect_tx(&ctl->sfull[ss], slab_bytes);
+                    tma_load_5d(s_smem + (size_t)ss * p.s_stage_bytes, tm, &ctl->sfull[ss], (int)P.c0, cw, ch,
+                                cd + pl * p.stride, t.nb);
                 }
                 if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
             }
@@ -459,11 +504,12 @@ conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
 
     if (warp >= kProducerWarp) {
         // ================================================================ producer warpgroup: one warp issues the TMA loads
-        setmaxnreg_dec<40>();
-        if (warp == kProducerWarp) produce_tiles(p, ctl, w_smem, s_smem, abort_flag, total_items);
+        // NV = 256 needs 232 consumer registers (a 128-register accumulator); narrower tiles leave the producer more
+        setmaxnreg_dec<NV == 256 ? 40 : 56>();
+        if (warp == kProducerWarp) produce_tiles_cm(p, ctl, w_smem, s_smem, abort_flag, total_items);
     } else {
         // ================================================================ consumers: warpgroup g computes plane d0 + g
-        setmaxnreg_inc<232>();
+        setmaxnreg_inc<NV == 256 ? 232 : 216>();
         const int g = warp >> 2, wq = warp & 3, wt = threadIdx.x & 127;
         float acc[NV / 2];
         int ws = 0, wph = 0, ss = 0, sph = 0;
@@ -519,19 +565,27 @@ conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
                 const bool f8 = P.f8 != 0;
                 if (prev_f8 >= 0 && prev_f8 != (int)f8) wgmma_wait<0>();
                 prev_f8 = (int)f8;
-                ok = mbar_wait(&ctl->wfull[ws], wph, abort_flag);
-                if (!ok) break;
-                const uint32_t w_addr = w_base0 + (uint32_t)(ws * p.w_stage_bytes);
+                // weight unit kd of this phase sits in ring stage w0 + kd (mod w_stages); slab pl is the last user of unit
+                // pl - tde + 1 (the plane-1 warpgroup reads unit kd at slab kd + 1), which is released with that slab
+                const int w0 = ws;
                 const int nplanes = t.tde + n_kd - 1;
                 for (int pl = 0; pl < nplanes && ok; ++pl) {
+                    if (pl < n_kd) {
+                        ok = mbar_wait(&ctl->wfull[ws], wph, abort_flag);
+                        if (!ok) break;
+                        if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
+                    }
                     ok = mbar_wait(&ctl->sfull[ss], sph, abort_flag);
                     if (!ok) break;
                     const int kd = pl - g;
                     int groups = 0;
                     if (has_plane && kd >= 0 && kd < n_kd) {
+                        int wsk = w0 + kd;
+                        if (wsk >= p.w_stages) wsk -= p.w_stages;
+                        const uint32_t w_addr = w_base0 + (uint32_t)(wsk * p.w_stage_bytes);
                         const uint32_t s_addr = s_base0 + (uint32_t)(ss * p.s_stage_bytes);
                         for (int kh = 0; kh < n_kh; ++kh) {
-                            const uint32_t a = w_addr + (uint32_t)((kh * n_kd + (n_kd - 1 - kd)) * 64 * 128);
+                            const uint32_t a = w_addr + (uint32_t)(kh * 64 * 128);
                             const uint32_t b = s_addr + (uint32_t)(kh * TW * 128);
                             if (f8) mma_block<NV, true>(acc, a, b);
                             else mma_block<NV, false>(acc, a, b);
@@ -541,11 +595,13 @@ conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
                     wgmma_wait_n(groups);          // the previous slab's MMAs have retired
                     release();
                     pend_s = ss;
+                    const int kd_done = pl - t.tde + 1;
+                    if (kd_done >= 0) {
+                        pend_w = w0 + kd_done;
+                        if (pend_w >= p.w_stages) pend_w -= p.w_stages;
+                    }
                     if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
                 }
-                pend_w = ws;
-                if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
-                if (p.w_stages == 1) { wgmma_wait<0>(); release(); }
             }
             wgmma_wait<0>();
             release();
@@ -848,9 +904,14 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     if ((int)slots.size() > kConvMaxSrc) return fail("too many (source, tap-class) slots");
     const std::vector<ConvPhase> phases = conv_build_phases(d);
     p.n_phases = (int)phases.size();
-    int max_taps = 1;
+    int max_taps = 1, max_kh = 1, max_kd = 1;
     bool any3 = false;
-    for (const auto& P : phases) { max_taps = std::max(max_taps, P.n_kh * P.n_kd); any3 |= (P.n_kh == 3); }
+    for (const auto& P : phases) {
+        max_taps = std::max(max_taps, P.n_kh * P.n_kd);
+        max_kh = std::max(max_kh, (int)P.n_kh);
+        max_kd = std::max(max_kd, (int)P.n_kd);
+        any3 |= (P.n_kh == 3);
+    }
 
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
@@ -938,7 +999,8 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     for (size_t i = 0; i < slots.size(); ++i) p.slab_rows[i] = p.TW * (p.TH + slots[i].n_kh - 1);
     int max_rows = 0;
     for (size_t i = 0; i < slots.size(); ++i) max_rows = std::max(max_rows, p.slab_rows[i]);
-    p.w_stage_bytes = max_taps * bn * 128;
+    // voxel-major: a weight stage holds all taps of a phase; channel-major: one kd tap (its n_kh tiles), see produce_tiles_cm
+    p.w_stage_bytes = (plan.channel_major ? max_kh : max_taps) * bn * 128;
     p.s_stage_bytes = max_rows * 128;
     // control block: barriers + per-warp statistics rows; the 1 KB alignment slack is dropped when exactly that buys
     // another slab stage (the kernel then verifies the base alignment itself)
@@ -948,6 +1010,15 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     const int ctl_core = kCtlBarrierBytes + (plan.channel_major ? 2 * kCmStageFloats * 4 : 0) + stats_bytes;
     auto plan_stages = [&](int slack, int& ws, int& ss) {
         const int avail = 227 * 1024 - ctl_core - slack;
+        if (plan.channel_major) {
+            // a phase holds all n_kd of its units at its middle slab, and the next phase's first unit must find a free stage
+            // while the last one is still in use when n_kd == 1; slab stages first (up to 6), then spare weight units
+            ws = std::max(2, max_kd);
+            if (ws * p.w_stage_bytes + 2 * p.s_stage_bytes > avail) return false;
+            ss = std::min(std::min(kMaxSStages, 6), (avail - ws * p.w_stage_bytes) / p.s_stage_bytes);
+            ws = std::min(kMaxWStages, (avail - ss * p.s_stage_bytes) / p.w_stage_bytes);
+            return true;
+        }
         ws = (2 * p.w_stage_bytes + 2 * p.s_stage_bytes <= avail) ? 2 : 1;
         if (ws * p.w_stage_bytes + 2 * p.s_stage_bytes > avail) return false;
         ss = std::min(std::min(kMaxSStages, 6), (avail - ws * p.w_stage_bytes) / p.s_stage_bytes);

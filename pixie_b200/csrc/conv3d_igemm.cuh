@@ -68,7 +68,7 @@ struct ConvKernelParams {
     int block_n;          // output channels per tile: 16 or 32 (voxel-major), 64 (channel-major)
     int n_tiles;          // ceil(Cout / block_n)
     // shared-memory plan
-    int w_stage_bytes, w_stages;   // weight stages (all taps of one phase)
+    int w_stage_bytes, w_stages;   // weight stages: all taps of one phase (voxel-major), one kd tap's n_kh tiles (channel-major)
     int s_stage_bytes, s_stages;   // slab stages
     int slab_rows[kConvMaxSrc];    // rows per slab for each source (TW * (TH + n_kh - 1))
     // epilogue
