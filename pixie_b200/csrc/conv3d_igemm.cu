@@ -115,6 +115,118 @@ __device__ __forceinline__ void wgmma_wait_n(int n) {
     }
 }
 
+// Position in a ring of stages: the stage and the parity of its barriers' current phase.
+struct RingPos {
+    int stage = 0, parity = 0;
+    __device__ __forceinline__ void advance(int n_stages) {
+        if (++stage == n_stages) { stage = 0; parity ^= 1; }
+    }
+};
+
+// Stages whose MMAs may still be in flight (-1: none). release() hands them back to the producer, one lane per consumer
+// warp arriving on their empty barriers, once the wgmma groups that read them have retired.
+struct PendingStages {
+    int s = -1, w = -1;
+    __device__ __forceinline__ void release(SmemCtrl* ctl, int lane) {
+        if (lane == 0) {
+            if (s >= 0) mbar_arrive(&ctl->sempty[s]);
+            if (w >= 0) mbar_arrive(&ctl->wempty[w]);
+        }
+        s = -1; w = -1;
+    }
+};
+
+// Fused output statistics of the consumer threads: per-channel sums gather in the CTA's shared-memory rows, scalar totals
+// (p.stats_scalar) in each thread's fp64 registers. Both fold into the global fp64 accumulators of batch item `nb` when the
+// consumers reach a tile of another item, and after their last tile.
+struct ConvStats {
+    float* rows;                 // [2][p.stats_ld]: sum, sum of squares
+    int nb = -1;
+    double tot_s = 0.0, tot_q = 0.0;
+
+    __device__ __forceinline__ void flush(const ConvKernelParams& p, int lane) {
+        if (p.stats_scalar) {
+            // totals go to channel 0's slot; the LayerNorm consumer sums the [Cout][2] row anyway
+#pragma unroll
+            for (int off = 16; off >= 1; off >>= 1) {
+                tot_s += __shfl_xor_sync(0xffffffffu, tot_s, off);
+                tot_q += __shfl_xor_sync(0xffffffffu, tot_q, off);
+            }
+            if (lane == 0) {
+                atomicAdd(p.stats + (size_t)nb * p.Cout * 2, tot_s);
+                atomicAdd(p.stats + (size_t)nb * p.Cout * 2 + 1, tot_q);
+            }
+            tot_s = 0.0; tot_q = 0.0;
+            return;
+        }
+        // both consumer warpgroups: fold the block's partial sums into the global fp64 accumulators
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        for (int ch = threadIdx.x; ch < p.Cout; ch += 256) {
+            atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2, (double)rows[ch]);
+            atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2 + 1, (double)rows[p.stats_ld + ch]);
+            rows[ch] = 0.f;
+            rows[p.stats_ld + ch] = 0.f;
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+    }
+    // before the epilogue of a tile of batch item item_nb
+    __device__ __forceinline__ void enter(const ConvKernelParams& p, int item_nb, int lane) {
+        if (nb != item_nb) {
+            if (nb >= 0) flush(p, lane);
+            nb = item_nb;
+        }
+    }
+};
+
+// Dynamic shared memory of both kernels: w_stages weight stages, s_stages slab stages, the control block (SmemCtrl in
+// kCtlBarrierBytes), the epilogue staging (channel-major), then the statistics rows (iff p.stats).
+struct ConvSmem {
+    uint8_t* w;
+    uint8_t* s;
+    SmemCtrl* ctl;
+    float* stage;
+    float* stats;
+};
+
+// Carves the dynamic shared memory (stage_floats of epilogue staging), initialises the barriers, prefetches the tensor maps
+// and clears the statistics rows; ends with a block-wide barrier.
+__device__ __forceinline__ ConvSmem conv_prologue(const ConvKernelParams& p, int stage_floats, int n_threads) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    // dynamic smem base is only guaranteed 16 B aligned by the ABI: align manually to 1024 B
+    uint8_t* smem = reinterpret_cast<uint8_t*>(
+        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+    ConvSmem m;
+    m.w = smem;
+    m.s = smem + (size_t)p.w_stages * p.w_stage_bytes;
+    m.ctl = reinterpret_cast<SmemCtrl*>(m.s + (size_t)p.s_stages * p.s_stage_bytes);
+    m.stage = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(m.ctl) + kCtlBarrierBytes);
+    m.stats = m.stage + stage_floats;
+    // plans without alignment slack (p.smem_slack == 0) rely on the 1 KB-aligned dynamic smem base that kernels without
+    // static shared memory get in practice; verified here, failing loudly through the error flag instead of corrupting smem
+    const bool smem_misaligned = (p.smem_slack == 0) && (smem != smem_raw);
+
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < kMaxWStages; ++i) { mbar_init(&m.ctl->wfull[i], 1); mbar_init(&m.ctl->wempty[i], kConsumerWarps); }
+        for (int i = 0; i < kMaxSStages; ++i) { mbar_init(&m.ctl->sfull[i], 1); mbar_init(&m.ctl->sempty[i], kConsumerWarps); }
+        m.ctl->abort_flag = smem_misaligned ? 1 : 0;
+        fence_barrier_init();
+    }
+    if ((threadIdx.x >> 5) == kProducerWarp && (threadIdx.x & 31) == 0) {
+        for (int i = 0; i < kConvMaxSrc; ++i) prefetch_tmap(&p.tmA[i]);
+        prefetch_tmap(&p.tmB);
+    }
+    if (p.stats != nullptr && !p.stats_scalar)
+        for (int i = threadIdx.x; i < 2 * p.stats_ld; i += n_threads) m.stats[i] = 0.f;
+    __syncthreads();
+    return m;
+}
+
+// Once every role has left its loop: a CTA whose pipeline aborted (timeout, or misaligned shared memory) reports itself.
+__device__ __forceinline__ void conv_report_abort(const ConvKernelParams& p, const SmemCtrl* ctl) {
+    __syncthreads();
+    if (threadIdx.x == 0 && ctl->abort_flag && p.err_flag) atomicExch(p.err_flag, 1 + (int)blockIdx.x);
+}
+
 // One input slab (input plane pl) of a phase, for this warpgroup's 64 rows: the slab feeds output planes d = pl - kd for the
 // kd taps of the phase, each through n_kh row-shifted views (kh taps). The accumulator of plane d is acc[d]. Returns the
 // number of wgmma groups committed.
@@ -128,7 +240,7 @@ __device__ __forceinline__ int issue_slab(float (&acc)[TD][BN / 2], uint32_t a_a
         const int kd = pl - d;
         for (int kh = 0; kh < n_kh; ++kh) {
             const uint32_t a = a_addr + (uint32_t)(kh * TW * 128);
-            const uint32_t b = w_addr + (uint32_t)((kh * n_kd + (n_kd - 1 - kd)) * BN * 128);
+            const uint32_t b = w_addr + (uint32_t)(conv_wtile(0, n_kd, kh, kd) * BN * 128);
             if (f8) mma_block<BN, true>(acc[d], a, b);
             else mma_block<BN, false>(acc[d], a, b);
             ++groups;
@@ -137,86 +249,51 @@ __device__ __forceinline__ int issue_slab(float (&acc)[TD][BN / 2], uint32_t a_a
     return groups;
 }
 
-// TMA producer loop (one warp; one elected lane issues): per tile and phase, the phase's weight tiles into a weight stage,
-// then the tde + n_kd - 1 input-plane slabs into the slab ring. Shared by both orientations, whose stages hold the same
-// rows (block_n weight rows per tap, TW x (TH + n_kh - 1) slab rows).
+// TMA producer loop (one warp; one elected lane issues). Per tile and phase, the tde + n_kd - 1 input-plane slabs go into the
+// slab ring and the phase's weight tiles into the weight ring in units of kUnitKd kd taps (kWholePhase: all n_kd taps, one
+// unit), unit u loaded just before slab u. Inside a unit over kd_lo .. kd_hi the tiles sit in the packed order, kh major,
+// then kd = kd_hi .. kd_lo.
+constexpr int kWholePhase = 0;
+
+template <int kUnitKd>
 __device__ __forceinline__ void produce_tiles(const ConvKernelParams& p, SmemCtrl* ctl, uint8_t* w_smem, uint8_t* s_smem,
                                               volatile int* abort_flag, int total_items) {
-    int ws = 0, wph = 0, ss = 0, sph = 0;
-    bool ok = true;
-    for (int wi = blockIdx.x; wi < total_items && ok; wi += gridDim.x) {
-        const TileCoord t = decode_tile(p, wi);
-        for (int ph = t.ph_begin; ph < t.ph_end && ok; ++ph) {
-            const ConvPhase P = p.phases[ph];
-            const int ntaps = P.n_kh * P.n_kd;
-            ok = mbar_wait(&ctl->wempty[ws], wph ^ 1, abort_flag);
-            if (!ok) break;
-            if (elect_one()) {
-                mbar_expect_tx(&ctl->wfull[ws], (uint32_t)(ntaps * p.block_n * 128));
-                uint8_t* wdst = w_smem + (size_t)ws * p.w_stage_bytes;
-                for (int tap = 0; tap < ntaps; ++tap)
-                    tma_load_2d(wdst + (size_t)tap * p.block_n * 128, &p.tmB, &ctl->wfull[ws],
-                                (P.wtile_base + tap) * 64, t.n0);
-            }
-            if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
-
-            const int nplanes = t.tde + P.n_kd - 1;
-            const uint32_t slab_bytes = (uint32_t)p.slab_rows[P.src] * 128u;
-            for (int pl = 0; pl < nplanes && ok; ++pl) {
-                ok = mbar_wait(&ctl->sempty[ss], sph ^ 1, abort_flag);
-                if (!ok) break;
-                if (elect_one()) {
-                    mbar_expect_tx(&ctl->sfull[ss], slab_bytes);
-                    tma_load_5d(s_smem + (size_t)ss * p.s_stage_bytes, &p.tmA[P.src],
-                                &ctl->sfull[ss], (int)P.c0, t.w0 * p.stride + P.dw,
-                                t.h0 * p.stride + P.dh0, (t.d0 + pl) * p.stride + P.dd0, t.nb);
-                }
-                if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
-            }
-        }
-    }
-}
-
-// Channel-major producer: the weight ring holds one kd tap of a phase per stage (its n_kh tiles, 24 KB for a 3x3x3 phase), loaded
-// just ahead of the first slab that uses it: unit kd before slab kd. A unit is released as soon as its last slab retires instead of
-// at the end of the phase, so three units take the place of two whole-phase stages and the freed 72 KB buy two more slab stages.
-__device__ __forceinline__ void produce_tiles_cm(const ConvKernelParams& p, SmemCtrl* ctl, uint8_t* w_smem, uint8_t* s_smem,
-                                                 volatile int* abort_flag, int total_items) {
-    int ws = 0, wph = 0, ss = 0, sph = 0;
+    RingPos wring, sring;
     bool ok = true;
     for (int wi = blockIdx.x; wi < total_items && ok; wi += gridDim.x) {
         const TileCoord t = decode_tile(p, wi);
         for (int ph = t.ph_begin; ph < t.ph_end && ok; ++ph) {
             const ConvPhase P = p.phases[ph];
             const int n_kd = P.n_kd, n_kh = P.n_kh, nplanes = t.tde + n_kd - 1;
-            const uint32_t slab_bytes = (uint32_t)p.slab_rows[P.src] * 128u, unit_bytes = (uint32_t)(n_kh * p.block_n * 128);
+            const int unit_kd = kUnitKd ? kUnitKd : n_kd, n_units = kUnitKd ? n_kd / kUnitKd : 1;
+            const uint32_t slab_bytes = (uint32_t)p.slab_rows[P.src] * 128u, unit_bytes = (uint32_t)(n_kh * unit_kd * p.block_n * 128);
             const CUtensorMap* tm = &p.tmA[P.src];
             const int cw = t.w0 * p.stride + P.dw, ch = t.h0 * p.stride + P.dh0, cd = t.d0 * p.stride + P.dd0;
-            // packed tile order inside a phase: kh major, then kd = n_kd - 1 .. 0; unit kd starts at tile n_kd - 1 - kd
-            int wcol = (P.wtile_base + n_kd - 1) * 64;
 #pragma unroll 1
             for (int pl = 0; pl < nplanes && ok; ++pl) {
-                if (pl < n_kd) {
-                    ok = mbar_wait(&ctl->wempty[ws], wph ^ 1, abort_flag);
+                if (pl < n_units) {
+                    ok = mbar_wait(&ctl->wempty[wring.stage], wring.parity ^ 1, abort_flag);
                     if (!ok) break;
                     if (elect_one()) {
-                        mbar_expect_tx(&ctl->wfull[ws], unit_bytes);
-                        uint8_t* wdst = w_smem + (size_t)ws * p.w_stage_bytes;
+                        mbar_expect_tx(&ctl->wfull[wring.stage], unit_bytes);
+                        uint8_t* wdst = w_smem + (size_t)wring.stage * p.w_stage_bytes;
+                        const int kd_lo = pl * unit_kd, kd_hi = kd_lo + unit_kd - 1;
 #pragma unroll 1
                         for (int kh = 0; kh < n_kh; ++kh)
-                            tma_load_2d(wdst + (size_t)kh * p.block_n * 128, &p.tmB, &ctl->wfull[ws], wcol + kh * n_kd * 64, t.n0);
+                            for (int kd = kd_hi; kd >= kd_lo; --kd)
+                                tma_load_2d(wdst + (size_t)conv_wtile(0, unit_kd, kh, kd - kd_lo) * p.block_n * 128, &p.tmB,
+                                            &ctl->wfull[wring.stage], conv_wtile(P.wtile_base, n_kd, kh, kd) * 64, t.n0);
                     }
-                    wcol -= 64;
-                    if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
+                    wring.advance(p.w_stages);
                 }
-                ok = mbar_wait(&ctl->sempty[ss], sph ^ 1, abort_flag);
+                ok = mbar_wait(&ctl->sempty[sring.stage], sring.parity ^ 1, abort_flag);
                 if (!ok) break;
                 if (elect_one()) {
-                    mbar_expect_tx(&ctl->sfull[ss], slab_bytes);
-                    tma_load_5d(s_smem + (size_t)ss * p.s_stage_bytes, tm, &ctl->sfull[ss], (int)P.c0, cw, ch,
+                    mbar_expect_tx(&ctl->sfull[sring.stage], slab_bytes);
+                    tma_load_5d(s_smem + (size_t)sring.stage * p.s_stage_bytes, tm, &ctl->sfull[sring.stage], (int)P.c0, cw, ch,
                                 cd + pl * p.stride, t.nb);
                 }
-                if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
+                sring.advance(p.s_stages);
             }
         }
     }
@@ -227,43 +304,18 @@ __device__ __forceinline__ void produce_tiles_cm(const ConvKernelParams& p, Smem
 template <int BN, int TD>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // dynamic smem base is only guaranteed 16 B aligned by the ABI: align manually to 1024 B
-    uint8_t* smem = reinterpret_cast<uint8_t*>(
-        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint8_t* w_smem = smem;
-    uint8_t* s_smem = smem + (size_t)p.w_stages * p.w_stage_bytes;
-    SmemCtrl* ctl = reinterpret_cast<SmemCtrl*>(s_smem + (size_t)p.s_stages * p.s_stage_bytes);
-    float* stats_sm = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ctl) + kCtlBarrierBytes);   // used iff p.stats
-    const int stats_ld = p.stats_ld;     // channels per statistics row (Cout rounded up to 32)
-    // plans without alignment slack (p.smem_slack == 0) rely on the 1 KB-aligned dynamic smem base that kernels without
-    // static shared memory get in practice; verified here, failing loudly through the error flag instead of corrupting smem
-    const bool smem_misaligned = (p.smem_slack == 0) && (smem != smem_raw);
-
+    const ConvSmem sm = conv_prologue(p, 0, kConvThreads);
+    SmemCtrl* ctl = sm.ctl;
+    volatile int* abort_flag = &ctl->abort_flag;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int total_items = p.NB * p.tiles_d * p.tiles_h * p.tiles_w * p.n_tiles * p.split_k;
+    const int total_items = conv_work_items(p.NB, p.tiles_d, p.tiles_h, p.tiles_w, p.n_tiles, p.split_k);
     const bool do_stats = p.stats != nullptr;
     const bool scalar_stats = do_stats && p.stats_scalar;     // consumer only needs the per-item totals (LayerNorm)
 
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < kMaxWStages; ++i) { mbar_init(&ctl->wfull[i], 1); mbar_init(&ctl->wempty[i], kConsumerWarps); }
-        for (int i = 0; i < kMaxSStages; ++i) { mbar_init(&ctl->sfull[i], 1); mbar_init(&ctl->sempty[i], kConsumerWarps); }
-        ctl->abort_flag = smem_misaligned ? 1 : 0;
-        fence_barrier_init();
-    }
-    if (warp == kProducerWarp && lane == 0) {
-        for (int i = 0; i < kConvMaxSrc; ++i) prefetch_tmap(&p.tmA[i]);
-        prefetch_tmap(&p.tmB);
-    }
-    if (do_stats && !scalar_stats)
-        for (int i = threadIdx.x; i < 2 * stats_ld; i += kConvThreads) stats_sm[i] = 0.f;
-    __syncthreads();
-    volatile int* abort_flag = &ctl->abort_flag;
-
     if (warp == kProducerWarp) {
         // ================================================================ TMA producer (warp-uniform, one elected lane issues)
-        produce_tiles(p, ctl, w_smem, s_smem, abort_flag, total_items);
+        produce_tiles<kWholePhase>(p, ctl, sm.w, sm.s, abort_flag, total_items);
     } else {
         // ================================================================ consumers: MMA + epilogue (warpgroups 0 and 1)
         // Each warpgroup owns rows 64 g .. 64 g + 63 of the 128-voxel plane tile and the TD plane accumulators of those rows in
@@ -271,38 +323,11 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
         // that the tensor cores always have the next slab's MMAs queued behind the current ones.
         const int g = warp >> 2, wq = warp & 3;
         float acc[TD][BN / 2];
-        int ws = 0, wph = 0, ss = 0, sph = 0;
-        const uint32_t w_base0 = smem_u32(w_smem), s_base0 = smem_u32(s_smem) + (uint32_t)(g * 64 * 128);
+        RingPos wring, sring;
+        const uint32_t w_base0 = smem_u32(sm.w), s_base0 = smem_u32(sm.s) + (uint32_t)(g * 64 * 128);
         bool ok = true;
         const long long DHW = (long long)p.D * p.H * p.W;
-        const int ct = threadIdx.x;             // 0..255 among the consumer threads
-        int stats_nb = -1;
-        double tot_s = 0.0, tot_q = 0.0;        // scalar statistics: this thread's running totals
-        auto flush_stats = [&](int nb) {
-            if (scalar_stats) {
-                // totals go to channel 0's slot; the LayerNorm consumer sums the [Cout][2] row anyway
-#pragma unroll
-                for (int off = 16; off >= 1; off >>= 1) {
-                    tot_s += __shfl_xor_sync(0xffffffffu, tot_s, off);
-                    tot_q += __shfl_xor_sync(0xffffffffu, tot_q, off);
-                }
-                if (lane == 0) {
-                    atomicAdd(p.stats + (size_t)nb * p.Cout * 2, tot_s);
-                    atomicAdd(p.stats + (size_t)nb * p.Cout * 2 + 1, tot_q);
-                }
-                tot_s = 0.0; tot_q = 0.0;
-                return;
-            }
-            // both consumer warpgroups: fold the block's partial sums into the global fp64 accumulators
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            for (int ch = ct; ch < p.Cout; ch += 256) {
-                atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2, (double)stats_sm[ch]);
-                atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2 + 1, (double)stats_sm[stats_ld + ch]);
-                stats_sm[ch] = 0.f;
-                stats_sm[stats_ld + ch] = 0.f;
-            }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-        };
+        ConvStats stats{sm.stats};
         // accumulator rows of this thread (the two rows of the wgmma fragment)
         int th2[2], tw2[2];
 #pragma unroll
@@ -318,15 +343,8 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
             for (int d = 0; d < TD; ++d)
 #pragma unroll
                 for (int j = 0; j < BN / 2; ++j) acc[d][j] = 0.f;
-            int pend_s = -1, pend_w = -1;       // stages whose MMAs may still be in flight
+            PendingStages pend;
             int prev_f8 = -1;                   // operand type of the previous phase of this tile
-            auto release = [&]() {
-                if (lane == 0) {
-                    if (pend_s >= 0) mbar_arrive(&ctl->sempty[pend_s]);
-                    if (pend_w >= 0) mbar_arrive(&ctl->wempty[pend_w]);
-                }
-                pend_s = -1; pend_w = -1;
-            };
             for (int ph = t.ph_begin; ph < t.ph_end && ok; ++ph) {
                 const ConvPhase P = p.phases[ph];
                 const int n_kd = P.n_kd, n_kh = P.n_kh;
@@ -334,27 +352,27 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
                 // wgmma groups of different shapes (E5M2 k32, fp16 k16) in flight on the same accumulators: drain at the switch
                 if (prev_f8 >= 0 && prev_f8 != (int)f8) wgmma_wait<0>();
                 prev_f8 = (int)f8;
-                ok = mbar_wait(&ctl->wfull[ws], wph, abort_flag);
+                ok = mbar_wait(&ctl->wfull[wring.stage], wring.parity, abort_flag);
                 if (!ok) break;
-                const uint32_t w_addr = w_base0 + (uint32_t)(ws * p.w_stage_bytes);
+                const uint32_t w_addr = w_base0 + (uint32_t)(wring.stage * p.w_stage_bytes);
                 const int nplanes = t.tde + n_kd - 1;
                 for (int pl = 0; pl < nplanes && ok; ++pl) {
-                    ok = mbar_wait(&ctl->sfull[ss], sph, abort_flag);
+                    ok = mbar_wait(&ctl->sfull[sring.stage], sring.parity, abort_flag);
                     if (!ok) break;
                     const int d_min = max(0, pl - (n_kd - 1)), d_max = min(t.tde - 1, pl);
-                    const int groups = issue_slab<BN, TD>(acc, s_base0 + (uint32_t)(ss * p.s_stage_bytes), w_addr, pl, d_min, d_max,
-                                                          n_kd, n_kh, p.TW, f8);
+                    const int groups = issue_slab<BN, TD>(acc, s_base0 + (uint32_t)(sring.stage * p.s_stage_bytes), w_addr, pl, d_min,
+                                                          d_max, n_kd, n_kh, p.TW, f8);
                     wgmma_wait_n(groups);          // the previous slab's MMAs have retired
-                    release();
-                    pend_s = ss;
-                    if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
+                    pend.release(ctl, lane);
+                    pend.s = sring.stage;
+                    sring.advance(p.s_stages);
                 }
-                pend_w = ws;
-                if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
-                if (p.w_stages == 1) { wgmma_wait<0>(); release(); }   // the producer needs this stage for the next phase
+                pend.w = wring.stage;
+                wring.advance(p.w_stages);
+                if (p.w_stages == 1) { wgmma_wait<0>(); pend.release(ctl, lane); }   // the producer needs this stage for the next phase
             }
             wgmma_wait<0>();
-            release();
+            pend.release(ctl, lane);
 #pragma unroll
             for (int d = 0; d < TD; ++d)
 #pragma unroll
@@ -362,10 +380,7 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
             if (!ok) break;
 
             // ---------------------------------------------------------------- epilogue from registers
-            if (do_stats && stats_nb != t.nb) {
-                if (stats_nb >= 0) flush_stats(stats_nb);
-                stats_nb = t.nb;
-            }
+            if (do_stats) stats.enter(p, t.nb, lane);
             const bool first_split = (t.split == 0);
             const bool use_bias = first_split && p.bias != nullptr;
             const bool use_res = first_split && p.residual != nullptr;
@@ -425,7 +440,7 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
                     for (int d = 0; d < TD; ++d)
 #pragma unroll
                         for (int j = 0; j < BN / 2; ++j) { s += acc[d][j]; q2 = fmaf(acc[d][j], acc[d][j], q2); }
-                    tot_s += (double)s; tot_q += (double)q2;
+                    stats.tot_s += (double)s; stats.tot_q += (double)q2;
                 } else {
                     // per column: this thread's rows and planes, then the 8 lanes holding the same columns
 #pragma unroll
@@ -447,118 +462,63 @@ conv3d_igemm_kernel(const __grid_constant__ ConvKernelParams p) {
                             }
                             const int ch = t.n0 + j8 * 8 + cq + e;
                             if (lane < 4 && ch < p.Cout) {
-                                atomicAdd(stats_sm + ch, s);
-                                atomicAdd(stats_sm + stats_ld + ch, q2);
+                                atomicAdd(stats.rows + ch, s);
+                                atomicAdd(stats.rows + p.stats_ld + ch, q2);
                             }
                         }
                 }
             }
         }
-        if (do_stats && stats_nb >= 0 && ok) flush_stats(stats_nb);
+        if (do_stats && stats.nb >= 0 && ok) stats.flush(p, lane);
     }
 
-    __syncthreads();
-    if (threadIdx.x == 0 && ctl->abort_flag && p.err_flag) atomicExch(p.err_flag, 1 + (int)blockIdx.x);
+    conv_report_abort(p, ctl);
 }
 
 // Channel-major instance: D[co][vox] = W[co][k] * S[vox][k]^T. A tile is 64 output channels x NV voxels (TH x TW of one plane)
 // x 2 planes; consumer warpgroup g owns output plane d0 + g, so one wgmma is m64 nNV (n256 for 16 x 16 tiles) and a slab
 // still feeds both warpgroups through its kd taps. The weight rows of a phase are the A operand, the slab rows the B operand;
-// the phase table, slab ring and barriers are those of the voxel-major kernel. The accumulator is NV / 2 registers per
-// thread: the producer warpgroup hands its registers to the two consumer warpgroups (setmaxnreg).
+// the phase table, producer, slab ring and barriers are those of the voxel-major kernel, but the weight ring holds one kd tap
+// per unit. The accumulator is NV / 2 registers per thread: the producer warpgroup hands its registers to the two consumer
+// warpgroups (setmaxnreg).
 template <int NV>
 __global__ void __launch_bounds__(kConvCmThreads, 1)
 conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
     constexpr int TW = NV == 64 ? 8 : 16;
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>(
-        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint8_t* w_smem = smem;
-    uint8_t* s_smem = smem + (size_t)p.w_stages * p.w_stage_bytes;
-    SmemCtrl* ctl = reinterpret_cast<SmemCtrl*>(s_smem + (size_t)p.s_stages * p.s_stage_bytes);
-    float* stage_sm = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ctl) + kCtlBarrierBytes);   // epilogue staging
-    float* stats_sm = stage_sm + 2 * kCmStageFloats;                                                   // used iff p.stats
-    const int stats_ld = p.stats_ld;
-    const bool smem_misaligned = (p.smem_slack == 0) && (smem != smem_raw);
-
+    const ConvSmem sm = conv_prologue(p, 2 * kCmStageFloats, kConvCmThreads);
+    SmemCtrl* ctl = sm.ctl;
+    volatile int* abort_flag = &ctl->abort_flag;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int total_items = p.NB * p.tiles_d * p.tiles_h * p.tiles_w * p.n_tiles * p.split_k;
+    const int total_items = conv_work_items(p.NB, p.tiles_d, p.tiles_h, p.tiles_w, p.n_tiles, p.split_k);
     const bool do_stats = p.stats != nullptr;
     const bool scalar_stats = do_stats && p.stats_scalar;
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < kMaxWStages; ++i) { mbar_init(&ctl->wfull[i], 1); mbar_init(&ctl->wempty[i], kConsumerWarps); }
-        for (int i = 0; i < kMaxSStages; ++i) { mbar_init(&ctl->sfull[i], 1); mbar_init(&ctl->sempty[i], kConsumerWarps); }
-        ctl->abort_flag = smem_misaligned ? 1 : 0;
-        fence_barrier_init();
-    }
-    if (warp == kProducerWarp && lane == 0) {
-        for (int i = 0; i < kConvMaxSrc; ++i) prefetch_tmap(&p.tmA[i]);
-        prefetch_tmap(&p.tmB);
-    }
-    if (do_stats && !scalar_stats)
-        for (int i = threadIdx.x; i < 2 * stats_ld; i += kConvCmThreads) stats_sm[i] = 0.f;
-    __syncthreads();
-    volatile int* abort_flag = &ctl->abort_flag;
 
     if (warp >= kProducerWarp) {
         // ================================================================ producer warpgroup: one warp issues the TMA loads
         // NV = 256 needs 232 consumer registers (a 128-register accumulator); narrower tiles leave the producer more
         setmaxnreg_dec<NV == 256 ? 40 : 56>();
-        if (warp == kProducerWarp) produce_tiles_cm(p, ctl, w_smem, s_smem, abort_flag, total_items);
+        if (warp == kProducerWarp) produce_tiles<1>(p, ctl, sm.w, sm.s, abort_flag, total_items);
     } else {
         // ================================================================ consumers: warpgroup g computes plane d0 + g
         setmaxnreg_inc<NV == 256 ? 232 : 216>();
         const int g = warp >> 2, wq = warp & 3, wt = threadIdx.x & 127;
         float acc[NV / 2];
-        int ws = 0, wph = 0, ss = 0, sph = 0;
-        const uint32_t w_base0 = smem_u32(w_smem), s_base0 = smem_u32(s_smem);
+        RingPos wring, sring;
+        const uint32_t w_base0 = smem_u32(sm.w), s_base0 = smem_u32(sm.s);
         bool ok = true;
-        const int ct = threadIdx.x;             // 0..255 among the consumer threads
-        int stats_nb = -1;
-        double tot_s = 0.0, tot_q = 0.0;
-        auto flush_stats = [&](int nb) {
-            if (scalar_stats) {
-#pragma unroll
-                for (int off = 16; off >= 1; off >>= 1) {
-                    tot_s += __shfl_xor_sync(0xffffffffu, tot_s, off);
-                    tot_q += __shfl_xor_sync(0xffffffffu, tot_q, off);
-                }
-                if (lane == 0) {
-                    atomicAdd(p.stats + (size_t)nb * p.Cout * 2, tot_s);
-                    atomicAdd(p.stats + (size_t)nb * p.Cout * 2 + 1, tot_q);
-                }
-                tot_s = 0.0; tot_q = 0.0;
-                return;
-            }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            for (int ch = ct; ch < p.Cout; ch += 256) {
-                atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2, (double)stats_sm[ch]);
-                atomicAdd(p.stats + ((size_t)nb * p.Cout + ch) * 2 + 1, (double)stats_sm[stats_ld + ch]);
-                stats_sm[ch] = 0.f;
-                stats_sm[stats_ld + ch] = 0.f;
-            }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-        };
+        ConvStats stats{sm.stats};
         // epilogue read-out: this thread's channel quad and voxel row inside a staged chunk
         const int q4 = wt & 15, vr = wt >> 4;
-        float* stage = stage_sm + g * kCmStageFloats;
+        float* stage = sm.stage + g * kCmStageFloats;
 
         for (int wi = blockIdx.x; wi < total_items && ok; wi += gridDim.x) {
             const TileCoord t = decode_tile(p, wi);
 #pragma unroll
             for (int j = 0; j < NV / 2; ++j) acc[j] = 0.f;
             const bool has_plane = g < t.tde;   // warpgroup-uniform
-            int pend_s = -1, pend_w = -1;
+            PendingStages pend;
             int prev_f8 = -1;
-            auto release = [&]() {
-                if (lane == 0) {
-                    if (pend_s >= 0) mbar_arrive(&ctl->sempty[pend_s]);
-                    if (pend_w >= 0) mbar_arrive(&ctl->wempty[pend_w]);
-                }
-                pend_s = -1; pend_w = -1;
-            };
             for (int ph = t.ph_begin; ph < t.ph_end && ok; ++ph) {
                 const ConvPhase P = p.phases[ph];
                 const int n_kd = P.n_kd, n_kh = P.n_kh;
@@ -567,15 +527,15 @@ conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
                 prev_f8 = (int)f8;
                 // weight unit kd of this phase sits in ring stage w0 + kd (mod w_stages); slab pl is the last user of unit
                 // pl - tde + 1 (the plane-1 warpgroup reads unit kd at slab kd + 1), which is released with that slab
-                const int w0 = ws;
+                const int w0 = wring.stage;
                 const int nplanes = t.tde + n_kd - 1;
                 for (int pl = 0; pl < nplanes && ok; ++pl) {
                     if (pl < n_kd) {
-                        ok = mbar_wait(&ctl->wfull[ws], wph, abort_flag);
+                        ok = mbar_wait(&ctl->wfull[wring.stage], wring.parity, abort_flag);
                         if (!ok) break;
-                        if (++ws == p.w_stages) { ws = 0; wph ^= 1; }
+                        wring.advance(p.w_stages);
                     }
-                    ok = mbar_wait(&ctl->sfull[ss], sph, abort_flag);
+                    ok = mbar_wait(&ctl->sfull[sring.stage], sring.parity, abort_flag);
                     if (!ok) break;
                     const int kd = pl - g;
                     int groups = 0;
@@ -583,9 +543,9 @@ conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
                         int wsk = w0 + kd;
                         if (wsk >= p.w_stages) wsk -= p.w_stages;
                         const uint32_t w_addr = w_base0 + (uint32_t)(wsk * p.w_stage_bytes);
-                        const uint32_t s_addr = s_base0 + (uint32_t)(ss * p.s_stage_bytes);
+                        const uint32_t s_addr = s_base0 + (uint32_t)(sring.stage * p.s_stage_bytes);
                         for (int kh = 0; kh < n_kh; ++kh) {
-                            const uint32_t a = w_addr + (uint32_t)(kh * 64 * 128);
+                            const uint32_t a = w_addr + (uint32_t)(conv_wtile(0, 1, kh, 0) * 64 * 128);
                             const uint32_t b = s_addr + (uint32_t)(kh * TW * 128);
                             if (f8) mma_block<NV, true>(acc, a, b);
                             else mma_block<NV, false>(acc, a, b);
@@ -593,18 +553,18 @@ conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
                         }
                     }
                     wgmma_wait_n(groups);          // the previous slab's MMAs have retired
-                    release();
-                    pend_s = ss;
+                    pend.release(ctl, lane);
+                    pend.s = sring.stage;
                     const int kd_done = pl - t.tde + 1;
                     if (kd_done >= 0) {
-                        pend_w = w0 + kd_done;
-                        if (pend_w >= p.w_stages) pend_w -= p.w_stages;
+                        pend.w = w0 + kd_done;
+                        if (pend.w >= p.w_stages) pend.w -= p.w_stages;
                     }
-                    if (++ss == p.s_stages) { ss = 0; sph ^= 1; }
+                    sring.advance(p.s_stages);
                 }
             }
             wgmma_wait<0>();
-            release();
+            pend.release(ctl, lane);
 #pragma unroll
             for (int j = 0; j < NV / 2; ++j) fence_operand(acc[j]);
             if (!ok) break;
@@ -612,10 +572,7 @@ conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
             // ---------------------------------------------------------------- epilogue through shared memory
             // The fragment holds 2 channels x NV / 4 voxels per thread; it is staged in chunks of kCmChunk voxels x 64
             // channels so that every output row is written (and the residual read) as 16-byte vectors.
-            if (do_stats && stats_nb != t.nb) {
-                if (stats_nb >= 0) flush_stats(stats_nb);
-                stats_nb = t.nb;
-            }
+            if (do_stats) stats.enter(p, t.nb, lane);
             if (!has_plane) continue;
             const bool first_split = (t.split == 0);
             const int ch = t.n0 + 4 * q4;
@@ -661,8 +618,8 @@ conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
             }
             if (do_stats) {
                 if (scalar_stats) {
-                    tot_s += (double)(st_s[0] + st_s[1] + st_s[2] + st_s[3]);
-                    tot_q += (double)(st_q[0] + st_q[1] + st_q[2] + st_q[3]);
+                    stats.tot_s += (double)(st_s[0] + st_s[1] + st_s[2] + st_s[3]);
+                    stats.tot_q += (double)(st_q[0] + st_q[1] + st_q[2] + st_q[3]);
                 } else {
                     // lanes q4 and q4 + 16 of a warp hold the same channels: one shuffle, then shared atomics
 #pragma unroll
@@ -673,18 +630,17 @@ conv3d_igemm_cm_kernel(const __grid_constant__ ConvKernelParams p) {
                     if (lane < 16 && ch_ok) {
 #pragma unroll
                         for (int i = 0; i < 4; ++i) {
-                            atomicAdd(stats_sm + ch + i, st_s[i]);
-                            atomicAdd(stats_sm + stats_ld + ch + i, st_q[i]);
+                            atomicAdd(stats.rows + ch + i, st_s[i]);
+                            atomicAdd(stats.rows + p.stats_ld + ch + i, st_q[i]);
                         }
                     }
                 }
             }
         }
-        if (do_stats && stats_nb >= 0 && ok) flush_stats(stats_nb);
+        if (do_stats && stats.nb >= 0 && ok) stats.flush(p, lane);
     }
 
-    __syncthreads();
-    if (threadIdx.x == 0 && ctl->abort_flag && p.err_flag) atomicExch(p.err_flag, 1 + (int)blockIdx.x);
+    conv_report_abort(p, ctl);
 }
 
 // =====================================================================================  host side
@@ -717,107 +673,93 @@ static int conv_slot_of(const std::vector<SrcSlot>& slots, int src, int n_kh) {
     return -1;
 }
 
-std::vector<ConvPhase> conv_build_phases(const ConvDesc& d) {
-    std::vector<ConvPhase> ph;
-    std::vector<int> rank;               // per phase: 0 E5M2 residual, 1 fp16 residual, 2 the main fp16 products
+// One phase as the host enumerates it: the kernel's ConvPhase and the segment it belongs to. The phase's n_kh x n_kd taps
+// are kernel taps (P.dd0 + pad + kd, P.dh0 + pad + kh, P.dw + pad), pad = ks / 2 of the segment; tap (kh, kd) sits in packed
+// weight tile conv_wtile(P.wtile_base, P.n_kd, kh, kd).
+struct PhaseRec {
+    ConvPhase P;
+    int seg;
+};
+
+// The phases of `d` in the kernel's order. Weight tiles are numbered segment by segment, then chunk, kw (and kh, kd for
+// stride-2 taps), before the phases are reordered: residual phases first, E5M2 ones before fp16 ones. The tensor cores do
+// not round the fp32 accumulation to nearest (and accumulate E5M2 products with a narrower mantissa still), so small
+// correction terms added to accumulators that already hold the main partial sums lose their low bits at every K step;
+// started from zero they keep their precision, and the main fp16 phases then accumulate on top.
+static std::vector<PhaseRec> conv_phase_records(const ConvDesc& d) {
+    std::vector<PhaseRec> recs;
     const auto slots = conv_src_slots(d);
     int wtile = 0;
-    for (const auto& s : d.segs) {
-        const ConvSrc& src = d.srcs[s.src];
-        const int chunks = src.C / 64;
-        if (s.ks == 1) {
-            for (int c = 0; c < chunks; ++c) {
-                ConvPhase P{};
-                P.src = (int8_t)conv_slot_of(slots, s.src, 1);
-                P.dw = 0; P.dh0 = 0; P.dd0 = 0; P.n_kh = 1; P.n_kd = 1;
-                P.c0 = (int16_t)(c * 64); P.wtile_base = wtile; wtile += 1; P.f8 = s.f8;
-                ph.push_back(P);
-            }
-        } else if (d.stride == 1) {
-            for (int c = 0; c < chunks; ++c)
-                for (int kw = 0; kw < 3; ++kw) {
-                    ConvPhase P{};
-                    P.src = (int8_t)conv_slot_of(slots, s.src, 3);
-                    P.dw = (int8_t)(kw - 1); P.dh0 = -1; P.dd0 = -1; P.n_kh = 3; P.n_kd = 3;
-                    P.c0 = (int16_t)(c * 64); P.wtile_base = wtile; wtile += 9; P.f8 = s.f8;
-                    ph.push_back(P);
-                }
-        } else {
-            for (int c = 0; c < chunks; ++c)
-                for (int kw = 0; kw < 3; ++kw)
-                    for (int kh = 0; kh < 3; ++kh)
-                        for (int kd = 0; kd < 3; ++kd) {
-                            ConvPhase P{};
-                            P.src = (int8_t)conv_slot_of(slots, s.src, 1);
-                            P.dw = (int8_t)(kw - 1); P.dh0 = (int8_t)(kh - 1); P.dd0 = (int8_t)(kd - 1);
-                            P.n_kh = 1; P.n_kd = 1;
-                            P.c0 = (int16_t)(c * 64); P.wtile_base = wtile; wtile += 1; P.f8 = s.f8;
-                            ph.push_back(P);
-                        }
-        }
-        rank.resize(ph.size(), s.f8 ? 0 : (s.lo || s.wlo) ? 1 : 2);
+    for (int si = 0; si < (int)d.segs.size(); ++si) {
+        const auto& s = d.segs[si];
+        const int chunks = d.srcs[s.src].C / 64;
+        // stride-1 3x3x3: one phase per (chunk, kw) holding all 9 (kd, kh) taps; otherwise one phase per tap
+        const int n_k = (s.ks == 3 && d.stride == 1) ? 3 : 1, n_ph = s.ks / n_k, pad = s.ks / 2;
+        for (int c = 0; c < chunks; ++c)
+            for (int kw = 0; kw < s.ks; ++kw)
+                for (int kh = 0; kh < n_ph; ++kh)
+                    for (int kd = 0; kd < n_ph; ++kd) {
+                        ConvPhase P{};
+                        P.src = (int8_t)conv_slot_of(slots, s.src, n_k);
+                        P.dw = (int8_t)(kw - pad);
+                        P.dh0 = (int8_t)(kh - pad);
+                        P.dd0 = (int8_t)(kd - pad);
+                        P.n_kh = (int8_t)n_k;
+                        P.n_kd = (int8_t)n_k;
+                        P.c0 = (int16_t)(c * 64);
+                        P.wtile_base = wtile;
+                        P.f8 = s.f8;
+                        wtile += n_k * n_k;
+                        recs.push_back({P, si});
+                    }
     }
-    // Residual phases first, E5M2 ones before fp16 ones: the tensor cores do not round the fp32 accumulation to nearest
-    // (and accumulate E5M2 products with a narrower mantissa still), so small correction terms added to accumulators that
-    // already hold the main partial sums lose their low bits at every K step; started from zero they keep their precision,
-    // and the main fp16 phases then accumulate on top. (Each phase carries its own weight tiles.)
-    std::vector<int> order(ph.size());
-    for (size_t i = 0; i < order.size(); ++i) order[i] = (int)i;
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return rank[a] < rank[b]; });
-    std::vector<ConvPhase> sorted;
-    for (int i : order) sorted.push_back(ph[i]);
-    return sorted;
+    auto rank = [&](const PhaseRec& r) {   // 0 E5M2 residual, 1 fp16 residual, 2 the main fp16 products
+        const auto& s = d.segs[r.seg];
+        return s.f8 ? 0 : (s.lo || s.wlo) ? 1 : 2;
+    };
+    std::stable_sort(recs.begin(), recs.end(), [&](const PhaseRec& a, const PhaseRec& b) { return rank(a) < rank(b); });
+    return recs;
+}
+
+std::vector<ConvPhase> conv_build_phases(const ConvDesc& d) {
+    std::vector<ConvPhase> ph;
+    for (const auto& r : conv_phase_records(d)) ph.push_back(r.P);
+    return ph;
 }
 
 void conv_pack_weights(const ConvDesc& d, const std::vector<const float*>& seg_weights,
                        const std::vector<int>& seg_cin_real, std::vector<__half>& packed) {
     const int K = conv_k_total(d);
     packed.assign((size_t)d.Cout_pad * K, __float2half(0.f));
-    int wtile = 0;
-    for (size_t si = 0; si < d.segs.size(); ++si) {
-        const auto& s = d.segs[si];
-        const ConvSrc& src = d.srcs[s.src];
-        const int chunks = src.C / 64;
-        const int cin = seg_cin_real[si];
-        const int ks = s.ks, kv = ks * ks * ks;
-        const float* w = seg_weights[si];   // [Cout][cin][kd][kh][kw]
-        const float up = (float)(1 << kF8Shift), down = 1.0f / up;
-        auto e5m2 = [](float v) { return (uint8_t)__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E5M2); };
-        auto put = [&](int tile, int c, int kd, int kh, int kw) {
-            for (int co = 0; co < d.Cout; ++co) {
-                // an f8 tile is 128 bytes per row: [e5m2(w / 2^s) x 64 | e5m2((w - fp16(w)) * 2^s) x 64]
-                uint8_t* row8 = reinterpret_cast<uint8_t*>(&packed[(size_t)co * K + (size_t)tile * 64]);
-                for (int cil = 0; cil < 64; ++cil) {
-                    const int ci = c * 64 + cil;
-                    if (ci >= cin) continue;
-                    float v = w[((size_t)co * cin + ci) * kv + (kd * ks + kh) * ks + kw];
-                    if (s.f8) {
-                        row8[cil] = e5m2(v * down);
-                        row8[64 + cil] = e5m2((v - __half2float(__float2half(v))) * up);
-                        continue;
+    const float up = (float)(1 << kF8Shift), down = 1.0f / up;
+    auto e5m2 = [](float v) { return (uint8_t)__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E5M2); };
+    for (const auto& r : conv_phase_records(d)) {
+        const ConvPhase& P = r.P;
+        const auto& s = d.segs[r.seg];
+        const int cin = seg_cin_real[r.seg];
+        const int ks = s.ks, kv = ks * ks * ks, pad = ks / 2;
+        const float* w = seg_weights[r.seg];   // [Cout][cin][kd][kh][kw]
+        for (int kh = 0; kh < P.n_kh; ++kh)
+            for (int kd = 0; kd < P.n_kd; ++kd) {
+                const int tile = conv_wtile(P.wtile_base, P.n_kd, kh, kd);
+                const int tap = ((P.dd0 + pad + kd) * ks + P.dh0 + pad + kh) * ks + P.dw + pad;
+                for (int co = 0; co < d.Cout; ++co) {
+                    // an f8 tile is 128 bytes per row: [e5m2(w / 2^s) x 64 | e5m2((w - fp16(w)) * 2^s) x 64]
+                    uint8_t* row8 = reinterpret_cast<uint8_t*>(&packed[(size_t)co * K + (size_t)tile * 64]);
+                    for (int cil = 0; cil < 64; ++cil) {
+                        const int ci = P.c0 + cil;
+                        if (ci >= cin) continue;
+                        float v = w[((size_t)co * cin + ci) * kv + tap];
+                        if (s.f8) {
+                            row8[cil] = e5m2(v * down);
+                            row8[64 + cil] = e5m2((v - __half2float(__float2half(v))) * up);
+                            continue;
+                        }
+                        if (s.wlo) v = v - __half2float(__float2half(v));
+                        packed[(size_t)co * K + (size_t)tile * 64 + cil] = __float2half(v);
                     }
-                    if (s.wlo) v = v - __half2float(__float2half(v));
-                    packed[(size_t)co * K + (size_t)tile * 64 + cil] = __float2half(v);
                 }
             }
-        };
-        if (ks == 1) {
-            for (int c = 0; c < chunks; ++c) put(wtile++, c, 0, 0, 0);
-        } else if (d.stride == 1) {
-            for (int c = 0; c < chunks; ++c)
-                for (int kw = 0; kw < 3; ++kw) {
-                    // tile order inside the phase: kh major, then kd = 2,1,0 (tile kh * 3 + 2 - kd, as the kernel's
-                    // issue_slab indexes it)
-                    for (int kd = 0; kd < 3; ++kd)
-                        for (int kh = 0; kh < 3; ++kh) put(wtile + kh * 3 + (2 - kd), c, kd, kh, kw);
-                    wtile += 9;
-                }
-        } else {
-            for (int c = 0; c < chunks; ++c)
-                for (int kw = 0; kw < 3; ++kw)
-                    for (int kh = 0; kh < 3; ++kh)
-                        for (int kd = 0; kd < 3; ++kd) put(wtile++, c, kd, kh, kw);
-        }
     }
 }
 
@@ -885,6 +827,86 @@ int conv_plan_retarget(const ConvDesc& d, ConvPlan& plan, char* err, int errlen)
     return encode_a_maps(d, plan.p, enc, err, errlen);
 }
 
+// Channel-major geometry: 64 output channels x NV voxels (TH x TW of one plane) x TD = 2 planes. A weight stage holds one kd
+// tap of a phase (its n_kh tiles). Returns an error message or nullptr.
+static const char* cm_geometry(const ConvDesc& d, int sms, int max_kh, ConvKernelParams& p) {
+    int nv = d.nv;
+    if (nv && nv != 64 && nv != 128 && nv != 256) return "bad nv";
+    if (!nv) {
+        // voxel tile: 16 x 16, 8 x 16 or 8 x 8 of one plane. Wave quantisation: a persistent grid of `sms` CTAs finishes in
+        // ceil(tiles/sms) rounds; prefer the tile with the best last-round fill times the share of real voxels, each halving
+        // of NV costing ~7 % (more weight and slab traffic per MAC, narrower MMAs)
+        double best = -1.0;
+        for (int v : {256, 128, 64}) {
+            if (v != 64 && d.W < 16) continue;
+            const int tw = v == 64 ? 8 : 16, th = v / tw;
+            const int tx = (d.W + tw - 1) / tw, ty = (d.H + th - 1) / th;
+            const long long tiles = conv_work_items(d.NB, (d.D + 1) / 2, ty, tx, (d.Cout_pad + 63) / 64, 1);
+            const long long rounds = (tiles + sms - 1) / sms;
+            const double sc = (double)tiles / (double)(rounds * sms) * (double)d.W * d.H / (double)(tx * tw * ty * th) *
+                              std::pow(0.93, v == 256 ? 0 : v == 128 ? 1 : 2);
+            if (sc > best) { best = sc; nv = v; }
+        }
+    }
+    p.TW = nv == 64 ? 8 : 16;
+    p.TH = nv / p.TW;
+    p.TD = 2;
+    p.block_n = 64;
+    p.w_stage_bytes = max_kh * p.block_n * 128;
+    return nullptr;
+}
+
+// Channel-major stages: a phase holds all n_kd of its weight units at its middle slab, and the next phase's first unit must
+// find a free stage while the last one is still in use when n_kd == 1; slab stages first (up to 6), then spare units.
+static bool cm_stages(const ConvKernelParams& p, int max_kd, int avail, int& ws, int& ss) {
+    ws = std::max(2, max_kd);
+    if (ws * p.w_stage_bytes + 2 * p.s_stage_bytes > avail) return false;
+    ss = std::min(std::min(kMaxSStages, 6), (avail - ws * p.w_stage_bytes) / p.s_stage_bytes);
+    ws = std::min(kMaxWStages, (avail - ss * p.s_stage_bytes) / p.w_stage_bytes);
+    return true;
+}
+
+// Voxel-major geometry: 128 voxels (TH x TW of one plane) x TD planes x block_n output channels. A weight stage holds all
+// taps of a phase. Returns an error message or nullptr.
+static const char* vm_geometry(const ConvDesc& d, int sms, bool any3, int max_taps, ConvKernelParams& p) {
+    p.TW = (d.W >= 16) ? 16 : 8;
+    p.TH = 128 / p.TW;
+    // N tile: 16 or 32; columns past Cout_pad are zero-filled by the weight TMA and never stored
+    int bn = d.block_n;
+    if (bn == 0) bn = d.Cout_pad > 16 ? 32 : 16;
+    if (bn != 16 && bn != 32) return "bad block_n";
+
+    // TD: output planes per tile. Their accumulators live in the consumer warpgroups' registers: TD * block_n <= 128
+    // fp32 columns (64 registers per thread).
+    int td = d.td ? d.td : std::min(4, 128 / bn);
+    td = std::max(1, std::min(td, d.D));
+    if (!any3 && !d.td) td = std::min(td, 2);    // no plane re-use without kd taps: smaller tiles, more CTAs (unless forced)
+    if (td == 3) td = 2;                // the kernel is instantiated for TD = 1, 2, 4
+    if (td * bn > 128) return "TD*block_n exceeds the register accumulator budget (128)";
+    if (!d.td && td > 1) {
+        // wave quantisation: prefer the plane count with the better last-round fill
+        auto fill = [&](int t) {
+            const long long tiles = conv_work_items(d.NB, (d.D + t - 1) / t, (d.H + p.TH - 1) / p.TH, (d.W + p.TW - 1) / p.TW,
+                                                    (d.Cout_pad + bn - 1) / bn, 1);
+            const long long rounds = (tiles + sms - 1) / sms;
+            return (double)tiles / (double)(rounds * sms) * (t == td ? 1.0 : 0.93);   // halving TD costs ~7 % more slab traffic
+        };
+        if (fill(td / 2) > fill(td)) td /= 2;
+    }
+    p.TD = td;
+    p.block_n = bn;
+    p.w_stage_bytes = max_taps * bn * 128;
+    return nullptr;
+}
+
+// Voxel-major stages: two whole-phase weight stages when they fit beside two slab stages, else one; then up to 6 slab stages.
+static bool vm_stages(const ConvKernelParams& p, int avail, int& ws, int& ss) {
+    ws = (2 * p.w_stage_bytes + 2 * p.s_stage_bytes <= avail) ? 2 : 1;
+    if (ws * p.w_stage_bytes + 2 * p.s_stage_bytes > avail) return false;
+    ss = std::min(std::min(kMaxSStages, 6), (avail - ws * p.w_stage_bytes) / p.s_stage_bytes);
+    return true;
+}
+
 int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* err, int errlen) {
     auto fail = [&](const char* m) { snprintf(err, errlen, "conv_plan_create: %s", m); return 1; };
     PFN_encodeTiled enc = get_encode_fn();
@@ -923,67 +945,15 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     // leave most of M empty, and planar outputs take the voxel-major kernel.
     plan.channel_major = d.Cout >= 64 && d.Cout % 4 == 0 && !d.out_planar && out_ld % 4 == 0 && d.out_c0 % 4 == 0 &&
                          reinterpret_cast<uintptr_t>(d.out) % 16 == 0 && reinterpret_cast<uintptr_t>(d.residual) % 16 == 0;
-    int bn = 0, td = 0, nv = 0;
-    if (plan.channel_major) {
-        bn = 64;
-        td = 2;
-        // voxel tile: 16 x 16, 8 x 16 or 8 x 8 of one plane. Wave quantisation: a persistent grid of `sms` CTAs finishes in
-        // ceil(tiles/sms) rounds; prefer the tile with the best last-round fill times the share of real voxels, each halving
-        // of NV costing ~7 % (more weight and slab traffic per MAC, narrower MMAs)
-        auto score = [&](int v, double& best) {
-            const int tw = v == 64 ? 8 : 16, th = v / tw;
-            const long long tx = (d.W + tw - 1) / tw, ty = (d.H + th - 1) / th;
-            const long long tiles = (long long)d.NB * tx * ty * ((d.D + 1) / 2) * ((d.Cout_pad + 63) / 64);
-            const long long rounds = (tiles + sms - 1) / sms;
-            const double sc = (double)tiles / (double)(rounds * sms) * (double)d.W * d.H / (double)(tx * tw * ty * th) *
-                              std::pow(0.93, v == 256 ? 0 : v == 128 ? 1 : 2);
-            if (sc > best) { best = sc; nv = v; }
-        };
-        if (d.nv) {
-            if (d.nv != 64 && d.nv != 128 && d.nv != 256) return fail("bad nv");
-            nv = d.nv;
-        } else {
-            double best = -1.0;
-            for (int v : {256, 128, 64})
-                if (v == 64 || d.W >= 16) score(v, best);
-        }
-        p.TW = nv == 64 ? 8 : 16;
-        p.TH = nv / p.TW;
-    } else {
-        p.TW = (d.W >= 16) ? 16 : 8;
-        p.TH = 128 / p.TW;
-        // N tile: 16 or 32; columns past Cout_pad are zero-filled by the weight TMA and never stored
-        bn = d.block_n;
-        if (bn == 0) bn = d.Cout_pad > 16 ? 32 : 16;
-        if (bn != 16 && bn != 32) return fail("bad block_n");
-
-        // TD: output planes per tile. Their accumulators live in the consumer warpgroups' registers: TD * block_n <= 128
-        // fp32 columns (64 registers per thread).
-        td = d.td ? d.td : std::min(4, 128 / bn);
-        td = std::max(1, std::min(td, d.D));
-        if (!any3 && !d.td) td = std::min(td, 2);    // no plane re-use without kd taps: smaller tiles, more CTAs (unless forced)
-        if (td == 3) td = 2;                // the kernel is instantiated for TD = 1, 2, 4
-        if (td * bn > 128) return fail("TD*block_n exceeds the register accumulator budget (128)");
-        if (!d.td && td > 1) {
-            // wave quantisation: prefer the plane count with the better last-round fill
-            auto fill = [&](int t) {
-                const long long tiles = (long long)d.NB * ((d.W + p.TW - 1) / p.TW) * ((d.H + p.TH - 1) / p.TH) * ((d.D + t - 1) / t) *
-                                        ((d.Cout_pad + bn - 1) / bn);
-                const long long rounds = (tiles + sms - 1) / sms;
-                return (double)tiles / (double)(rounds * sms) * (t == td ? 1.0 : 0.93);   // halving TD costs ~7 % more slab traffic
-            };
-            if (fill(td / 2) > fill(td)) td /= 2;
-        }
-    }
-    p.block_n = bn;
-    p.n_tiles = (d.Cout_pad + bn - 1) / bn;
-    p.TD = td;
+    const char* bad = plan.channel_major ? cm_geometry(d, sms, max_kh, p) : vm_geometry(d, sms, any3, max_taps, p);
+    if (bad) return fail(bad);
+    p.n_tiles = (d.Cout_pad + p.block_n - 1) / p.block_n;
     p.tiles_w = (d.W + p.TW - 1) / p.TW;
     p.tiles_h = (d.H + p.TH - 1) / p.TH;
     p.tiles_d = (d.D + p.TD - 1) / p.TD;
 
     // split-K
-    const int items = d.NB * p.tiles_w * p.tiles_h * p.tiles_d * p.n_tiles;
+    const int items = conv_work_items(d.NB, p.tiles_d, p.tiles_h, p.tiles_w, p.n_tiles, 1);
     int split = d.split_k;
     if (split <= 0) {
         split = 1;
@@ -999,8 +969,6 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     for (size_t i = 0; i < slots.size(); ++i) p.slab_rows[i] = p.TW * (p.TH + slots[i].n_kh - 1);
     int max_rows = 0;
     for (size_t i = 0; i < slots.size(); ++i) max_rows = std::max(max_rows, p.slab_rows[i]);
-    // voxel-major: a weight stage holds all taps of a phase; channel-major: one kd tap (its n_kh tiles), see produce_tiles_cm
-    p.w_stage_bytes = (plan.channel_major ? max_kh : max_taps) * bn * 128;
     p.s_stage_bytes = max_rows * 128;
     // control block: barriers + per-warp statistics rows; the 1 KB alignment slack is dropped when exactly that buys
     // another slab stage (the kernel then verifies the base alignment itself)
@@ -1010,19 +978,7 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
     const int ctl_core = kCtlBarrierBytes + (plan.channel_major ? 2 * kCmStageFloats * 4 : 0) + stats_bytes;
     auto plan_stages = [&](int slack, int& ws, int& ss) {
         const int avail = 227 * 1024 - ctl_core - slack;
-        if (plan.channel_major) {
-            // a phase holds all n_kd of its units at its middle slab, and the next phase's first unit must find a free stage
-            // while the last one is still in use when n_kd == 1; slab stages first (up to 6), then spare weight units
-            ws = std::max(2, max_kd);
-            if (ws * p.w_stage_bytes + 2 * p.s_stage_bytes > avail) return false;
-            ss = std::min(std::min(kMaxSStages, 6), (avail - ws * p.w_stage_bytes) / p.s_stage_bytes);
-            ws = std::min(kMaxWStages, (avail - ss * p.s_stage_bytes) / p.w_stage_bytes);
-            return true;
-        }
-        ws = (2 * p.w_stage_bytes + 2 * p.s_stage_bytes <= avail) ? 2 : 1;
-        if (ws * p.w_stage_bytes + 2 * p.s_stage_bytes > avail) return false;
-        ss = std::min(std::min(kMaxSStages, 6), (avail - ws * p.w_stage_bytes) / p.s_stage_bytes);
-        return true;
+        return plan.channel_major ? cm_stages(p, max_kd, avail, ws, ss) : vm_stages(p, avail, ws, ss);
     };
     int ws1 = 0, ss1 = 0, ws0 = 0, ss0 = 0;
     const bool ok1 = plan_stages(1024, ws1, ss1), ok0 = plan_stages(0, ws0, ss0);
@@ -1037,7 +993,7 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
         const int K = conv_k_total(d);
         cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)d.Cout_pad};
         cuuint64_t gstr[1] = {(cuuint64_t)K * 2};
-        cuuint32_t box[2] = {64, (cuuint32_t)bn};
+        cuuint32_t box[2] = {64, (cuuint32_t)p.block_n};
         cuuint32_t estr[2] = {1, 1};
         CUresult r = enc(&p.tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)d.weights, gdim, gstr, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -1059,7 +1015,7 @@ int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* e
 
     plan.grid = std::min(items * split, sms);
 
-    plan.kernel = plan.channel_major ? conv_cm_kernel_for(nv) : conv_kernel_for(bn, td);
+    plan.kernel = plan.channel_major ? conv_cm_kernel_for(p.TH * p.TW) : conv_kernel_for(p.block_n, p.TD);
     plan.threads = plan.channel_major ? kConvCmThreads : kConvThreads;
     if (cudaFuncSetAttribute(plan.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
         return fail("cudaFuncSetAttribute(max dynamic smem)");
@@ -1071,15 +1027,15 @@ void conv_plan_destroy(ConvPlan& plan) {
     plan.d_phases = nullptr;
 }
 
-int conv_plan_launch(const ConvPlan& plan, cudaStream_t stream) {
-    if (plan.needs_zero) {
-        // split-K accumulates with red.add: only the channel slice written by this conv may be
-        // cleared when out_ld > Cout, so callers with sliced outputs must not use split-K.
-        // Sized by the launched batch (p.NB), which callers may lower below the planned one: `out` then holds only
-        // p.NB items, and clearing the planned count would write past its end.
-        cudaMemsetAsync(plan.p.out, 0, plan.out_item_bytes * (size_t)plan.p.NB, stream);
-    }
-    plan.kernel<<<plan.grid, plan.threads, plan.smem_bytes, stream>>>(plan.p);
+int conv_plan_launch(const ConvPlan& plan, int nb, cudaStream_t stream) {
+    if (nb < 1 || nb > plan.p.NB) return (int)cudaErrorInvalidValue;
+    ConvKernelParams p = plan.p;
+    p.NB = nb;
+    const int grid = std::min(plan.grid, conv_work_items(nb, p.tiles_d, p.tiles_h, p.tiles_w, p.n_tiles, p.split_k));
+    // split-K accumulates with red.add: only the channel slice written by this conv may be cleared when out_ld > Cout, so
+    // callers with sliced outputs must not use split-K. `out` holds the launched items only: clear those.
+    if (plan.needs_zero) cudaMemsetAsync(p.out, 0, plan.out_item_bytes * (size_t)nb, stream);
+    plan.kernel<<<grid, plan.threads, plan.smem_bytes, stream>>>(p);
     return (int)cudaGetLastError();
 }
 

@@ -19,13 +19,15 @@
 //
 // The K loop is organised in PHASES so that shared memory, not L2, serves the tap re-use:
 //   phase = (source tensor, 64-channel chunk, kw)  for 3x3x3 stride-1 convolutions.
-// For one phase the CTA keeps the 9 (kd,kh) weight tiles resident and marches over the TD+2 input
-// planes of its tile; every plane slab ((TH+2) x TW voxels x 64 ch, loaded once by TMA with
-// zero-fill for the padding) feeds up to 9 MMAs: kh shifts are 1024 B-aligned row offsets into the
-// slab (TW is a multiple of 8 rows of 128 B), kd shifts select which of the TD accumulators the MMA
-// targets. kw needs its own slab copy because a one-voxel shift along w is not a multiple of the
-// 8-row swizzle atom.  1x1x1 convolutions (projector, ResBlock skip, attention qkv/proj) and
-// stride-2 taps are phases with n_kh = n_kd = 1.
+// For one phase the CTA marches over the TD+2 input planes of its tile; every plane slab ((TH+2) x TW
+// voxels x 64 ch, loaded once by TMA with zero-fill for the padding) feeds up to 9 MMAs: kh shifts are
+// 1024 B-aligned row offsets into the slab (TW is a multiple of 8 rows of 128 B), kd shifts select the
+// output plane the MMA targets. kw needs its own slab copy because a one-voxel shift along w is not a
+// multiple of the 8-row swizzle atom.  1x1x1 convolutions (projector, ResBlock skip, attention
+// qkv/proj) and stride-2 taps are phases with n_kh = n_kd = 1.
+// The phase's 9 (kd,kh) weight tiles reach shared memory in UNITS of whole kd taps, unit u loaded
+// just before slab u: voxel-major keeps all of them resident as one unit per phase, channel-major
+// rings one kd tap (its n_kh tiles) per unit and releases it as soon as its last slab retires.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -52,6 +54,17 @@ struct ConvPhase {        // 16 bytes, lives in global memory
     int32_t f8;           // 1: operands are E5M2 bytes (128 per row instead of 64 halfs), issued as wgmma .e5m2 (K = 32)
 };
 static_assert(sizeof(ConvPhase) == 16, "ConvPhase layout");
+
+// Packed weight tile (64 K-columns) of tap (kh, kd) of a phase whose tiles start at wtile_base: kh major, then
+// kd = n_kd - 1 .. 0, so that the kd taps a slab feeds are adjacent.
+__host__ __device__ __forceinline__ int conv_wtile(int wtile_base, int n_kd, int kh, int kd) {
+    return wtile_base + kh * n_kd + (n_kd - 1 - kd);
+}
+
+// Work items of a launch: one per (batch item, tile, channel tile, split-K range).
+__host__ __device__ __forceinline__ int conv_work_items(int nb, int tiles_d, int tiles_h, int tiles_w, int n_tiles, int split_k) {
+    return nb * tiles_d * tiles_h * tiles_w * n_tiles * split_k;
+}
 
 struct ConvKernelParams {
     CUtensorMap tmA[kConvMaxSrc];
@@ -149,13 +162,15 @@ struct ConvPlan {
     int smem_bytes = 0;
     bool needs_zero = false;   // out must be zeroed before launch (atomic_out)
     bool fused_stats = false;  // the epilogue accumulates ConvDesc::stats (needs split_k == 1, Cout <= 256)
-    size_t out_item_bytes = 0; // bytes of `out` per batch item; a split-K launch clears p.NB of them
+    size_t out_item_bytes = 0; // bytes of `out` per batch item; a split-K launch clears the launched items' share
 };
 
 // Returns 0 on success; on failure returns non-zero and fills `err`.
 int conv_plan_create(const ConvDesc& d, int* d_err_flag, ConvPlan& plan, char* err, int errlen);
 void conv_plan_destroy(ConvPlan& plan);
-int conv_plan_launch(const ConvPlan& plan, cudaStream_t stream);
+// Launches the plan for the first nb batch items (1 <= nb <= the planned batch; `out` need only hold those): fewer
+// items only shrink the tile count. Returns 0 or a CUDA error code.
+int conv_plan_launch(const ConvPlan& plan, int nb, cudaStream_t stream);
 // Re-encode the activation tensor maps after the source pointers in `d` changed (same shapes).
 int conv_plan_retarget(const ConvDesc& d, ConvPlan& plan, char* err, int errlen);
 }  // namespace pixie

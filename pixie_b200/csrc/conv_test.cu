@@ -57,7 +57,7 @@ struct Case {
     bool timing = false;
     int prec = kF16;
     int stats = kChanStats;                // statistics requested from the epilogue
-    int launch_nb = 0;                     // > 0: planned for NB items, launched with p.NB lowered to this (as the executor does)
+    int launch_nb = 0;                     // > 0: planned for NB items, launched for this many (as the executor does)
 };
 
 struct Totals {
@@ -187,17 +187,11 @@ static bool run_case(const Case& c, int* d_err, Totals& T) {
         cleanup();
         return false;
     }
-    ConvPlan pl = plan;                                   // as launched: the executor's lowering of NB and the grid
-    if (nl != NB) {
-        pl.p.NB = nl;
-        const int items = nl * pl.p.tiles_d * pl.p.tiles_h * pl.p.tiles_w * pl.p.n_tiles * pl.p.split_k;
-        pl.grid = std::min(items, pl.grid);
-    }
-    const std::string inst = pl.channel_major ? "cm(" + std::to_string(pl.p.TH * pl.p.TW) + ")"
-                                              : "vm(" + std::to_string(pl.p.block_n) + "," + std::to_string(pl.p.TD) + ")";
-    printf("[%s] %s NB=%d launched=%d grid=%d smem=%d %s bn=%d TD=%d TW=%d TH=%d w_stages=%d s_stages=%d phases=%d split=%d stats=%s%s\n",
-           c.name.c_str(), kPrecName[c.prec], NB, nl, pl.grid, pl.smem_bytes, inst.c_str(), pl.p.block_n, pl.p.TD, pl.p.TW, pl.p.TH,
-           pl.p.w_stages, pl.p.s_stages, pl.p.n_phases, pl.p.split_k, kStatsName[c.stats], plan.fused_stats ? " (fused)" : "");
+    const std::string inst = plan.channel_major ? "cm(" + std::to_string(plan.p.TH * plan.p.TW) + ")"
+                                                : "vm(" + std::to_string(plan.p.block_n) + "," + std::to_string(plan.p.TD) + ")";
+    printf("[%s] %s NB=%d launched=%d plan_grid=%d smem=%d %s bn=%d TD=%d TW=%d TH=%d w_stages=%d s_stages=%d phases=%d split=%d stats=%s%s\n",
+           c.name.c_str(), kPrecName[c.prec], NB, nl, plan.grid, plan.smem_bytes, inst.c_str(), plan.p.block_n, plan.p.TD, plan.p.TW, plan.p.TH,
+           plan.p.w_stages, plan.p.s_stages, plan.p.n_phases, plan.p.split_k, kStatsName[c.stats], plan.fused_stats ? " (fused)" : "");
     fflush(stdout);
     bool plan_ok = true;
     const std::string want = c.nv ? "cm(" + std::to_string(c.nv) + ")"
@@ -206,9 +200,9 @@ static bool run_case(const Case& c, int* d_err, Totals& T) {
         printf("[%s] forced %s but the plan uses %s\n", c.name.c_str(), want.c_str(), inst.c_str());
         plan_ok = false;
     }
-    if (c.want_split && pl.p.split_k == 1) { printf("[%s] expected a split-K plan\n", c.name.c_str()); plan_ok = false; }
+    if (c.want_split && plan.p.split_k == 1) { printf("[%s] expected a split-K plan\n", c.name.c_str()); plan_ok = false; }
 
-    const int lrc = conv_plan_launch(pl, 0);
+    const int lrc = conv_plan_launch(plan, nl, 0);
     const cudaError_t se = cudaDeviceSynchronize();
     int h_err = 0;
     cudaMemcpy(&h_err, d_err, sizeof(int), cudaMemcpyDeviceToHost);
@@ -224,7 +218,7 @@ static bool run_case(const Case& c, int* d_err, Totals& T) {
     if (c.timing) {
         cudaEvent_t e0, e1;
         cudaEventCreate(&e0); cudaEventCreate(&e1);
-        for (int i = 0; i < 3; ++i) conv_plan_launch(pl, 0);
+        for (int i = 0; i < 3; ++i) conv_plan_launch(plan, nl, 0);
         const int iters = 20;
         float ms = 0;
         if (getenv("CONV_TEST_COLD")) {
@@ -234,14 +228,14 @@ static bool run_case(const Case& c, int* d_err, Totals& T) {
             for (int i = 0; i < iters; ++i) {
                 CK(cudaMemsetAsync(scrub, i, 512u << 20, 0));
                 cudaEventRecord(e0);
-                conv_plan_launch(pl, 0);
+                conv_plan_launch(plan, nl, 0);
                 cudaEventRecord(e1);
                 CK(cudaEventSynchronize(e1));
                 float t = 0; cudaEventElapsedTime(&t, e0, e1); ms += t;
             }
         } else {
             cudaEventRecord(e0);
-            for (int i = 0; i < iters; ++i) conv_plan_launch(pl, 0);
+            for (int i = 0; i < iters; ++i) conv_plan_launch(plan, nl, 0);
             cudaEventRecord(e1);
             CK(cudaEventSynchronize(e1));
             cudaEventElapsedTime(&ms, e0, e1);
@@ -259,6 +253,15 @@ static bool run_case(const Case& c, int* d_err, Totals& T) {
         const uint8_t* gb = reinterpret_cast<const uint8_t*>(h_out.data() + out_elems);
         for (size_t i = 0; i < guard * 4; ++i) guard_bad += gb[i] != 0xA5;
     }
+    {
+        // FNV-1a over the output bytes, so that two builds can be compared bit for bit. Plain stores after a fixed MMA order
+        // make it reproducible; split-K reduces with red.add in arrival order, so its outputs (and the statistics) are not.
+        uint64_t hash = 1469598103934665603ull;
+        const uint8_t* ob = reinterpret_cast<const uint8_t*>(h_out.data());
+        for (size_t i = 0; i < out_elems * 4; ++i) hash = (hash ^ ob[i]) * 1099511628211ull;
+        printf("[%s] OUTHASH %016llx%s\n", c.name.c_str(), (unsigned long long)hash,
+               plan.p.split_k > 1 ? " (split-K: not deterministic)" : "");
+    }
 
     // ---- voxels to check: all, or (large cases) every voxel on an edge of its tile (at least two of its d, h, w on the
     // first or last index of the tile or of the volume) plus random ones
@@ -272,7 +275,7 @@ static bool run_case(const Case& c, int* d_err, Totals& T) {
         std::mt19937 g2(99);
         for (size_t v = 0; v < (size_t)nl * vout; ++v) {
             const int w = (int)(v % Do), h = (int)(v / Do % Do), dd = (int)(v / ((size_t)Do * Do) % Do);
-            const int n_edge = edge(dd, pl.p.TD) + edge(h, pl.p.TH) + edge(w, pl.p.TW);
+            const int n_edge = edge(dd, plan.p.TD) + edge(h, plan.p.TH) + edge(w, plan.p.TW);
             if (n_edge >= 2 || g2() % 4096 == 0) vs.push_back(v);
         }
     }

@@ -231,14 +231,8 @@ struct Builder {
         if (conv_plan_create(d, u.d_err, op->plan, e, sizeof(e))) { fail(e); return nullptr; }
         ConvOp* raw = op.get();
         UNet* up = &u;
-        u.ops.push_back([=](cudaStream_t st) {
-            // the plan was built for NBmax; smaller batches only shrink the tile count
-            ConvPlan pl = raw->plan;
-            pl.p.NB = up->cur_nb;
-            const int items = pl.p.NB * pl.p.tiles_d * pl.p.tiles_h * pl.p.tiles_w * pl.p.n_tiles * pl.p.split_k;
-            pl.grid = items < pl.grid ? items : pl.grid;
-            return conv_plan_launch(pl, st);
-        });
+        // the plan was built for NBmax; smaller batches only shrink the tile count
+        u.ops.push_back([=](cudaStream_t st) { return conv_plan_launch(raw->plan, up->cur_nb, st); });
         u.op_kinds.push_back(PIXIE_OP_CONV); u.op_flops.push_back(u.flops - flops_before);
         const bool fused = raw->plan.fused_stats;
         u.convs.push_back(std::move(op));
