@@ -123,6 +123,26 @@ int pixie_particle_volume(const float* pos_dev, int n, int grid_n, float grid_dx
 int pixie_frame_transform(const float* pos_dev, const float* cov_dev, int n, float z_shift_value, float scale_origin,
                           const float original_mean_pos_host[3], const float* rotations_host, int n_rot, float* pos_out_dev,
                           float* cov_out_dev, void* stream);
+/* ---- particle filling of hollow Gaussian objects (PG/particle_filling/filling.py:26-380, Taichi in the reference).
+ * pixie_fill_density: densify_grids (:26-87). count_dev [grid_n^3] int32 = Gaussians per cell (a Gaussian outside the grid
+ * counts in the nearest border cell; the reference indexes out of range), density_dev [grid_n^3] fp32 = sum over the
+ * Gaussians of opacity * the mean over the cell's 8 corner nodes of exp(-1/2 d^T P d), P = Q diag(1/max(sig, 1e-8)) Q^T from
+ * the signed eigen-decomposition of the covariance, over the (2r+1)^3 cells around the Gaussian's cell that lie in the grid,
+ * r = ceil(max sqrt(sig) / grid_dx). pos [n][3] in the grid's frame, opacity [n], cov [n][6] upper triangle. Both grids are
+ * overwritten; C order (x slowest). */
+int pixie_fill_density(const float* pos_dev, const float* opacity_dev, const float* cov_dev, int n, int grid_n, float grid_dx,
+                       int* count_dev, float* density_dev, void* stream);
+/* pixie_fill_grids: fill_dense_grids (:90-114) then internal_filling (:117-234) on the grids of pixie_fill_density. A cell
+ * with density > density_thres and count < max_particles_per_cell gets the difference; then every cell whose count is still
+ * 0, that sees a cell with density > search_thres in each axis direction other than exclude_dir (0 +x, 1 -x, 2 +y, 3 -y,
+ * 4 +z, 5 -z) and an odd number of such runs along ray_cast_dir, gets max_particles_per_cell. count_dev is updated in place
+ * like the reference's grid. New particles (cell + U[0,1)^3) * grid_dx + origin go to out_dev [max_samples][3]: dense-cell
+ * ones first, each group in C order of cells, offsets from Philox keyed on (seed, output index). *n_dense_host /
+ * *n_total_host receive the counts (the call synchronises `stream` once); a total above max_samples fails and writes nothing
+ * to out_dev. */
+int pixie_fill_grids(int* count_dev, const float* density_dev, int grid_n, float grid_dx, const float origin_host[3],
+                     float density_thres, float search_thres, int max_particles_per_cell, int exclude_dir, int ray_cast_dir,
+                     unsigned long long seed, float* out_dev, int max_samples, int* n_dense_host, int* n_total_host, void* stream);
 /* Number of kernel launches one forward() issues (for gpu_launches accounting) and algorithmic
  * FLOPs of one forward at batch 1 (2 * MACs of every Conv3d/Conv1d of the reference graph). */
 int pixie_unet_launch_count(pixie_unet_t h);

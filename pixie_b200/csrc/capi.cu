@@ -5,6 +5,7 @@
 #include "unet_kernels.cuh"
 #include "field_transfer.cuh"
 #include "cluster.cuh"
+#include "particle_fill.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -132,6 +133,34 @@ int pixie_frame_transform(const float* pos, const float* cov, int n, float z_shi
     if (n_rot < 0 || n_rot > 8) return set_err("frame_transform: at most 8 rotations");
     if (require_device()) return 1;
     if (pixie::frame_transform(pos, cov, n, z_shift, scale, mean, rotations, n_rot, pos_out, cov_out, (cudaStream_t)stream)) return set_err("frame_transform failed");
+    return 0;
+}
+// n^3 cells and their offsets are int32 on the device
+static bool fill_grid_ok(int grid_n) { return grid_n >= 1 && grid_n <= 1290; }
+int pixie_fill_density(const float* pos, const float* opacity, const float* cov, int n, int grid_n, float grid_dx, int* count, float* density,
+                       void* stream) {
+    if (!count || !density || (n > 0 && (!pos || !opacity || !cov))) return set_err("null argument");
+    if (n < 0 || !fill_grid_ok(grid_n) || !(grid_dx > 0.f)) return set_err("fill_density: need n >= 0, 1 <= grid_n <= 1290 and grid_dx > 0");
+    if (require_device()) return 1;
+    if (pixie::fill_density(pos, opacity, cov, n, grid_n, grid_dx, count, density, (cudaStream_t)stream)) return set_err("fill_density failed");
+    return 0;
+}
+int pixie_fill_grids(int* count, const float* density, int grid_n, float grid_dx, const float origin[3], float density_thres, float search_thres,
+                     int max_particles_per_cell, int exclude_dir, int ray_cast_dir, unsigned long long seed, float* out, int max_samples,
+                     int* n_dense_host, int* n_total_host, void* stream) {
+    if (!count || !density || !origin || !n_dense_host || !n_total_host || (max_samples > 0 && !out)) return set_err("null argument");
+    if (!fill_grid_ok(grid_n) || !(grid_dx > 0.f)) return set_err("fill_grids: need 1 <= grid_n <= 1290 and grid_dx > 0");
+    if (max_particles_per_cell < 1 || (long long)grid_n * grid_n * grid_n * max_particles_per_cell > 2147483647LL)
+        return set_err("fill_grids: need 1 <= max_particles_per_cell and grid_n^3 * max_particles_per_cell < 2^31");
+    if (exclude_dir < 0 || exclude_dir > 5 || ray_cast_dir < 0 || ray_cast_dir > 5) return set_err("fill_grids: directions must be in 0..5");
+    if (max_samples < 0) return set_err("fill_grids: negative max_samples");
+    if (require_device()) return 1;
+    const int rc = pixie::fill_grids(count, density, grid_n, grid_dx, origin, density_thres, search_thres, max_particles_per_cell, exclude_dir,
+                                     ray_cast_dir, seed, out, max_samples, n_dense_host, n_total_host, (cudaStream_t)stream);
+    if (rc == 3)
+        return set_err("fill_grids: filling adds " + std::to_string(*n_total_host) + " particles (" + std::to_string(*n_dense_host) +
+                       " in dense cells) but max_samples is " + std::to_string(max_samples));
+    if (rc) return set_err("fill_grids failed");
     return 0;
 }
 int pixie_pack_predictions(const float* seg_logits_dev, const float* cont_dev, float* out_dev, int batch, int64_t voxels, int n_classes, void* stream) {

@@ -9,6 +9,7 @@ per scene, none of it arithmetic. Here the two networks and one solver stay resi
 
     grid (fp16 NDHWC .npy or tensor) --predict_packed_host_stream--> (3+8, D,D,D) field     [inference_combined.py:122-199]
     field + mask --extract_material_points--> material point cloud (the PLY's vertex table)   [map_pred_to_coords.py:128-283]
+    Gaussians --fill_particles, when the scene has a particle_filling block-->                [gs_simulation.py:442-462]
     particles --get_particle_volume / load_initial_data / set_parameters_dict / BCs-->        [gs_simulation.py:464-489]
     kNN smoothing (+ ground / stationary cuboids) + upload (apply_material_field_to_simulation) [material_field.py:295-550]
     frame loop: export positions / covariances in the Gaussians' frame, step_per_frame x p2g2p [gs_simulation.py:585-634]
@@ -26,7 +27,7 @@ from typing import Callable, Dict, Iterable, List, Optional, Sequence
 import numpy as np
 import torch
 
-from . import dist_utils, frame_export, material_transfer, voxel_io
+from . import dist_utils, frame_export, material_transfer, particle_filling, voxel_io
 from .inference import MaterialFieldPredictor
 from .mpm_solver_warp import MPM_Simulator_WARP
 
@@ -54,6 +55,9 @@ class Scene:
     material_field_bcs: bool = False
     fix_ground: bool = True
     only_handle_largest_cluster: bool = True
+    opacity: Optional[torch.Tensor] = None         # (N,) or (N, 1) opacities; needed by particle filling
+    # the config's `particle_filling` block (decode_param.py:177-208 defaults applied here); None simulates the Gaussians only
+    particle_filling: Optional[Dict] = None
 
 
 def transform2origin(position_tensor: torch.Tensor):
@@ -144,7 +148,6 @@ class SceneBatchDriver:
         rotated = apply_rotations(sc.particles.to(dev, torch.float32), rots)
         transformed, scale_origin, original_mean_pos = transform2origin(rotated)
         pos0 = transformed + torch.tensor([1.0, 1.0, 1.0 + sc.z_shift_value], device=dev)          # shift2center111 :103-105
-        vol = frame_export.get_particle_volume(pos0, n_grid, grid_lim / n_grid, unifrom=mp.get("material") == "sand")
         cov0 = None
         if sc.cov is not None:
             # apply_cov_rotations(init_cov, R) * scale^2  (gs_simulation.py:438): R C R^T per rotation, on the device
@@ -153,6 +156,10 @@ class SceneBatchDriver:
             for R in rots:
                 m = R @ m @ R.T
             cov0 = torch.stack([m[:, 0, 0], m[:, 0, 1], m[:, 0, 2], m[:, 1, 1], m[:, 1, 2], m[:, 2, 2]], dim=1) * (scale_origin ** 2)
+        gs_num = int(pos0.shape[0])
+        if sc.particle_filling is not None:
+            pos0, cov0 = self._fill(sc, pos0, cov0, n_grid, grid_lim)
+        vol = frame_export.get_particle_volume(pos0, n_grid, grid_lim / n_grid, unifrom=mp.get("material") == "sand")
         solver = MPM_Simulator_WARP(10, device=str(dev))
         solver.load_initial_data_from_torch(pos0, vol, cov0, n_grid=n_grid, grid_lim=grid_lim, device=str(dev))
         solver.set_parameters_dict(mp, device=str(dev))
@@ -172,9 +179,12 @@ class SceneBatchDriver:
         substep_dt = tp["substep_dt"]
         step_per_frame = int(tp["frame_dt"] / substep_dt)                                           # float division like :627
         frames_pos, frames_cov = [], []
+        filled = gs_num != int(pos0.shape[0])
         for frame in range(int(tp["frame_num"])):
             pos = solver.export_particle_x_to_torch()
             cov = solver.export_particle_cov_to_torch().view(-1, 6) if sc.cov is not None else None
+            if filled:                                                                             # the Gaussians only (:591, 594)
+                pos, cov = pos[:gs_num], cov[:gs_num]
             pr, cr = frame_export.render_frame_transform(pos, cov, sc.z_shift_value, scale_origin, original_mean_pos, rots)
             if on_frame is not None:
                 on_frame(frame, pr, cr)
@@ -182,9 +192,27 @@ class SceneBatchDriver:
                 frames_pos.append(pr.clone())
                 frames_cov.append(None if cr is None else cr.clone())
             solver.p2g2p_n(step_per_frame, substep_dt)
-        return {"name": sc.name, "n_particles": int(pos0.shape[0]), "frames_pos": frames_pos, "frames_cov": frames_cov,
+        return {"name": sc.name, "n_particles": int(pos0.shape[0]), "n_gaussians": gs_num, "frames_pos": frames_pos, "frames_cov": frames_cov,
                 "material_ids": props[4], "E": props[2], "substeps": step_per_frame * int(tp["frame_num"]), "time": solver.time,
                 "bc_conditions": bc_conditions}
+
+    def _fill(self, sc: Scene, pos0: torch.Tensor, cov0: Optional[torch.Tensor], n_grid: int, grid_lim: float):
+        """Particle filling of gs_simulation.py:442-462, 479-480: the Gaussians first, then the filled particles with
+        covariance 0."""
+        fp = particle_filling.decode_filling_params(sc.particle_filling, {"n_grid": n_grid})
+        if fp["smooth"] or fp["visualize"]:
+            raise NotImplementedError(
+                f"scene {sc.name}: particle filling with smooth / visualize needs mcubes.smooth (PyMCubes), which is not available")
+        if sc.opacity is None or cov0 is None:
+            raise ValueError(f"scene {sc.name}: particle filling needs the Gaussians' opacity and cov")
+        pos = particle_filling.fill_particles(
+            pos=pos0, opacity=sc.opacity.to(self.device, torch.float32), cov=cov0, grid_n=fp["n_grid"], max_samples=fp["max_particles_num"],
+            grid_dx=grid_lim / fp["n_grid"], density_thres=fp["density_threshold"], search_thres=fp["search_threshold"],
+            max_particles_per_cell=fp["max_partciels_per_cell"], search_exclude_dir=fp["search_exclude_direction"],
+            ray_cast_dir=fp["ray_cast_direction"], boundary=fp["boundary"], smooth=False)
+        cov = torch.zeros((pos.shape[0], 6), dtype=torch.float32, device=pos.device)
+        cov[:pos0.shape[0]] = cov0
+        return pos, cov
 
     # ------------------------------------------------------------------------------ batch
     def run(self, scenes: Sequence[Scene], out_dir: Optional[str] = None) -> List[Dict]:
