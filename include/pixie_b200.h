@@ -231,6 +231,9 @@ typedef struct {
 } pixie_mpm_bc;
 
 int pixie_mpm_create(int n_particles, int n_grid, float grid_lim, pixie_mpm_t* out);
+/* bind, set_params, add_bc, clear_bcs, set_time / get_time, set_active_count and the slab set-up write pending results
+ * back and copy on the legacy default stream, which does not wait for non-blocking streams: a caller that steps on such a
+ * stream calls pixie_mpm_sync(h, stream) and synchronises that stream first (pixie_b200.mpm_solver_warp does). */
 int pixie_mpm_bind(pixie_mpm_t h, int field, void* dev_ptr);
 int pixie_mpm_set_params(pixie_mpm_t h, const pixie_mpm_params* p);
 int pixie_mpm_add_bc(pixie_mpm_t h, const pixie_mpm_bc* bc);

@@ -620,13 +620,17 @@ int mpm_add_bc(Mpm* m, const pixie_mpm_bc& b) {
     cudaMemcpy(m->d_bcs + k, &d, sizeof(DevBC), cudaMemcpyHostToDevice);
     cudaMemcpy(m->pts + 3 * k, d.point, 3 * sizeof(float), cudaMemcpyHostToDevice);
     cudaMemcpy(m->pts + (size_t)kMaxBC * 3 + 3 * k, d.point, 3 * sizeof(float), cudaMemcpyHostToDevice);
+    // a pageable host-to-device cudaMemcpy may return before its DMA lands, and the next substep may run on a stream
+    // that does not wait for the legacy one
+    cudaStreamSynchronize(0);
     m->graph_valid = false;
     return 0;
 }
 int mpm_clear_bcs(Mpm* m) { m->bcs.clear(); m->graph_valid = false; return 0; }
 int mpm_set_time(Mpm* m, double t) {
     const double both[2] = {t, t};
-    return cudaMemcpy(m->tslots, both, sizeof(both), cudaMemcpyHostToDevice) != cudaSuccess;
+    // synchronised like the copies of mpm_add_bc
+    return cudaMemcpy(m->tslots, both, sizeof(both), cudaMemcpyHostToDevice) != cudaSuccess || cudaStreamSynchronize(0) != cudaSuccess;
 }
 int mpm_get_time(Mpm* m, double* t) {
     const double* src = m->tslots + m->tpar;

@@ -172,6 +172,17 @@ class MPM_Simulator_WARP:
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self._device).cuda_stream)
 
+    def _fence(self, write_back=True):
+        """Puts a call that changes bindings, parameters, boundary conditions or the clock behind the substeps queued on
+        the caller's stream. Those C calls copy on the legacy default stream, which does not wait for torch's side
+        streams (they are non-blocking), so pending results are written back on the caller's stream and the host waits
+        for it first. Once the write-back is done, binding a field or setting parameters only changes host state, so the
+        wait is stricter than those two need; it is kept as the one rule for every such call, which only runs at set-up
+        and between rollouts."""
+        if write_back:
+            _lib.check(_lib.load().pixie_mpm_sync(self._handle, self._stream()))
+        torch.cuda.current_stream(self._device).synchronize()
+
     @property
     def _t(self):
         """Particle / model tensors in the caller's order. The default native path keeps a cell-sorted private copy
@@ -184,6 +195,7 @@ class MPM_Simulator_WARP:
 
     def _bind(self, fid: str, t: torch.Tensor):
         self._tensors[fid] = t
+        self._fence()
         _lib.check(_lib.load().pixie_mpm_bind(self._handle, _lib.FIELDS[fid], C.c_void_p(t.data_ptr())))
 
     def _push_params(self):
@@ -196,6 +208,7 @@ class MPM_Simulator_WARP:
         p.alpha, p.hardening, p.xi = float(m.alpha), float(m.hardening), float(m.xi)
         p.plastic_viscosity, p.softening = float(m.plastic_viscosity), float(m.softening)
         p.update_cov_with_F = int(bool(m.update_cov_with_F))
+        self._fence()
         _lib.check(_lib.load().pixie_mpm_set_params(self._handle, C.byref(p)))
 
     # simulation clock: `self.time` is a host float in the reference (:167, :637); here it lives on the
@@ -203,11 +216,13 @@ class MPM_Simulator_WARP:
     @property
     def time(self) -> float:
         t = C.c_double()
+        self._fence(write_back=False)
         _lib.check(_lib.load().pixie_mpm_get_time(self._handle, C.byref(t)))
         return t.value
 
     @time.setter
     def time(self, value: float):
+        self._fence(write_back=False)
         _lib.check(_lib.load().pixie_mpm_set_time(self._handle, float(value)))
 
     # ------------------------------------------------------------------------------ loading
@@ -409,6 +424,7 @@ class MPM_Simulator_WARP:
         if mask is not None:
             self._masks.append(mask)
             bc.mask_dev = C.c_void_p(mask.data_ptr())
+        self._fence()
         _lib.check(_lib.load().pixie_mpm_add_bc(self._handle, C.byref(bc)))
         self.n_bcs += 1
         return bc

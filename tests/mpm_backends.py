@@ -134,6 +134,21 @@ class OracleSolver:
                       rotation_scale=rotation_scale, translation_scale=translation_scale, start_time=start_time,
                       end_time=end_time, mask=mask)
 
+    def release_particles_sequentially(self, normal, start_position, end_position, num_layers, start_time, end_time):
+        num_layers = 50                                    # overridden like the reference (:1183-1210)
+        point, size, axis = [0, 0, 0], [0, 0, 0], -1
+        for i in range(3):
+            if normal[i] == 0:
+                point[i], size[i] = 1, 1
+            else:
+                axis, point[i] = i, end_position
+        half_length_portion = abs(start_position - end_position) / num_layers
+        end_time_portion = end_time / num_layers
+        for i in range(num_layers):
+            size[axis] = half_length_portion * (num_layers - i)
+            self.enforce_particle_velocity_translation(point=list(point), size=list(size), velocity=[0, 0, 0],
+                                                       start_time=start_time, end_time=end_time_portion * (i + 1))
+
     def export_particle_R_to_torch(self, device="cpu"):
         self.o.compute_R_from_F()
         return torch.from_numpy(self.o.get("R").reshape(-1, 9))
