@@ -143,6 +143,25 @@ int pixie_fill_density(const float* pos_dev, const float* opacity_dev, const flo
 int pixie_fill_grids(int* count_dev, const float* density_dev, int grid_n, float grid_dx, const float origin_host[3],
                      float density_thres, float search_thres, int max_particles_per_cell, int exclude_dir, int ray_cast_dir,
                      unsigned long long seed, float* out_dev, int max_samples, int* n_dense_host, int* n_total_host, void* stream);
+/* ---- Gaussian-splatting rasteriser, forward only (gs_simulation.py:573-631 with `--render_img`: Inria's
+ * diff-gaussian-rasterization at scale_modifier 1, prefiltered false, precomputed 3D covariances).
+ * A renderer keeps its device buffers between frames and grows them when a frame needs more; once warm, a frame allocates
+ * nothing. pixie_gs_render draws one frame on `stream`: means_dev [n][3], cov_dev [n][6] (upper triangle xx xy xz yy yz zz,
+ * the solver's export order), opacity_dev [n]; colours from shs_dev [n][sh_coeffs][3] evaluated at degree sh_degree (<= 3,
+ * (sh_degree + 1)^2 <= sh_coeffs) toward campos as utils/render_utils.py:113-130 does (+0.5, clamped at 0), or, when
+ * shs_dev is NULL, colors_dev [n][3] as given. view / proj: world_view_transform and full_proj_transform as the reference
+ * stores them (16 floats each, row-vector convention). image_dev [3][height][width] receives the unclamped RGB image over
+ * bg, radii_dev [n] the screen radius (0 = culled). The call synchronises `stream` once, for the number of (Gaussian, tile)
+ * pairs, which goes to *n_rendered_host (may be NULL). phase_ms_host, when not NULL, receives the times in ms of preprocess,
+ * scan + keys, sort, ranges and blend (CUDA events; the call then synchronises a second time). */
+typedef struct pixie_gs_renderer_s* pixie_gs_renderer_t;
+int pixie_gs_renderer_create(pixie_gs_renderer_t* out);
+int pixie_gs_render(pixie_gs_renderer_t h, const float* means_dev, const float* cov_dev, const float* opacity_dev,
+                    const float* shs_dev, int sh_coeffs, int sh_degree, const float* colors_dev, int n, const float view_host[16],
+                    const float proj_host[16], const float campos_host[3], float tan_fovx, float tan_fovy, int width, int height,
+                    const float bg_host[3], float* image_dev, int* radii_dev, int* n_rendered_host, float* phase_ms_host,
+                    void* stream);
+void pixie_gs_renderer_destroy(pixie_gs_renderer_t h);
 /* Number of kernel launches one forward() issues (for gpu_launches accounting) and algorithmic
  * FLOPs of one forward at batch 1 (2 * MACs of every Conv3d/Conv1d of the reference graph). */
 int pixie_unet_launch_count(pixie_unet_t h);

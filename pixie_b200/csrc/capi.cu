@@ -6,6 +6,7 @@
 #include "field_transfer.cuh"
 #include "cluster.cuh"
 #include "particle_fill.cuh"
+#include "gs_render.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -18,6 +19,7 @@ int set_err(const std::string& e) { g_err = e; return 1; }
 
 struct pixie_unet_s { pixie::UNet* u; };
 struct pixie_mpm_s { pixie::Mpm* m; };
+struct pixie_gs_renderer_s { pixie::GsRenderer* r; };
 
 extern "C" {
 
@@ -162,6 +164,43 @@ int pixie_fill_grids(int* count, const float* density, int grid_n, float grid_dx
                        " in dense cells) but max_samples is " + std::to_string(max_samples));
     if (rc) return set_err("fill_grids failed");
     return 0;
+}
+// ------------------------------------------------------------------------------------- Gaussian rasteriser
+int pixie_gs_renderer_create(pixie_gs_renderer_t* out) {
+    if (!out) return set_err("null argument");
+    if (require_device()) return 1;
+    pixie::GsRenderer* r = pixie::gs_renderer_create();
+    if (!r) return set_err("gs_renderer_create: out of memory");
+    *out = new pixie_gs_renderer_s{r};
+    return 0;
+}
+int pixie_gs_render(pixie_gs_renderer_t h, const float* means, const float* cov, const float* opacity, const float* shs, int sh_coeffs,
+                    int sh_degree, const float* colors, int n, const float view[16], const float proj[16], const float campos[3],
+                    float tan_fovx, float tan_fovy, int width, int height, const float bg[3], float* image, int* radii, int* n_rendered,
+                    float* phase_ms, void* stream) {
+    if (!h) return set_err("null handle");
+    if (!view || !proj || !campos || !bg || !image || (n > 0 && (!means || !cov || !opacity || !radii || (!shs && !colors))))
+        return set_err("null argument");
+    if (n < 0) return set_err("gs_render: negative Gaussian count");
+    if (width < 1 || height < 1 || (long long)width * height > 2147483647LL) return set_err("gs_render: bad image size");
+    if (!(tan_fovx > 0.f) || !(tan_fovy > 0.f)) return set_err("gs_render: tan(fov) must be positive");
+    if (shs && (sh_degree < 0 || sh_degree > 3 || (sh_degree + 1) * (sh_degree + 1) > sh_coeffs))
+        return set_err("gs_render: need 0 <= sh_degree <= 3 and (sh_degree + 1)^2 <= sh_coeffs");
+    pixie::GsRenderArgs a{};
+    a.means = means; a.cov = cov; a.opacity = opacity; a.shs = shs; a.colors = shs ? nullptr : colors;
+    a.n = n; a.sh_coeffs = sh_coeffs; a.sh_degree = sh_degree;
+    std::memcpy(a.view, view, sizeof(a.view));
+    std::memcpy(a.proj, proj, sizeof(a.proj));
+    std::memcpy(a.campos, campos, sizeof(a.campos));
+    std::memcpy(a.bg, bg, sizeof(a.bg));
+    a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy; a.width = width; a.height = height; a.image = image; a.radii = radii;
+    if (pixie::gs_render(h->r, a, n_rendered, phase_ms, (cudaStream_t)stream)) return set_err(pixie::gs_error(h->r));
+    return 0;
+}
+void pixie_gs_renderer_destroy(pixie_gs_renderer_t h) {
+    if (!h) return;
+    pixie::gs_renderer_destroy(h->r);
+    delete h;
 }
 int pixie_pack_predictions(const float* seg_logits_dev, const float* cont_dev, float* out_dev, int batch, int64_t voxels, int n_classes, void* stream) {
     if (!seg_logits_dev || !cont_dev || !out_dev) return set_err("null argument");

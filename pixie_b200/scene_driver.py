@@ -13,8 +13,10 @@ per scene, none of it arithmetic. Here the two networks and one solver stay resi
     particles --get_particle_volume / load_initial_data / set_parameters_dict / BCs-->        [gs_simulation.py:464-489]
     kNN smoothing (+ ground / stationary cuboids) + upload (apply_material_field_to_simulation) [material_field.py:295-550]
     frame loop: export positions / covariances in the Gaussians' frame, step_per_frame x p2g2p [gs_simulation.py:585-634]
+    + the rendered frame, when the scene has SH coefficients and camera parameters         [gs_simulation.py:573-619]
 
-Function names and argument meaning follow those reference functions; rendering, Hydra and the file layout stay outside.
+Function names and argument meaning follow those reference functions; image / video files, Hydra and the file layout stay
+outside.
 Scenes shard over ranks like the reference's `DistributedSampler(shuffle=False)` (dist_utils.shard_scenes); there is no
 data-path collective.
 """
@@ -27,7 +29,7 @@ from typing import Callable, Dict, Iterable, List, Optional, Sequence
 import numpy as np
 import torch
 
-from . import dist_utils, frame_export, material_transfer, particle_filling, voxel_io
+from . import dist_utils, frame_export, gs_render, material_transfer, particle_filling, voxel_io
 from .inference import MaterialFieldPredictor
 from .mpm_solver_warp import MPM_Simulator_WARP
 
@@ -58,6 +60,13 @@ class Scene:
     opacity: Optional[torch.Tensor] = None         # (N,) or (N, 1) opacities; needed by particle filling
     # the config's `particle_filling` block (decode_param.py:177-208 defaults applied here); None simulates the Gaussians only
     particle_filling: Optional[Dict] = None
+    # rendering (gs_simulation.py --render_img): with both `shs` and `camera_params`, every frame is rendered from the
+    # scene's own opacity and SH coefficients; otherwise nothing is rendered
+    shs: Optional[torch.Tensor] = None             # (N, 16, 3) SH coefficients, as GaussianModel.get_features
+    sh_degree: int = 3                             # the model's active SH degree
+    camera_params: Optional[Dict] = None           # the config's camera keys, raw or decode_camera_params'd
+    cameras: object = None                         # the model's cameras.json list, or its path
+    white_bg: bool = False
 
 
 def transform2origin(position_tensor: torch.Tensor):
@@ -138,9 +147,12 @@ class SceneBatchDriver:
 
     # ------------------------------------------------------------------------------ physics half
     def run_physics_simulation(self, sc: Scene, cloud: Dict[str, torch.Tensor],
-                               on_frame: Optional[Callable[[int, torch.Tensor, Optional[torch.Tensor]], None]] = None) -> Dict:
-        """One scene's rollout (gs_simulation.py:395-634 without the rasteriser): returns the per-frame render-space positions
-        (and covariances when the scene has them) unless `on_frame(frame, pos, cov)` consumes them."""
+                               on_frame: Optional[Callable[[int, torch.Tensor, Optional[torch.Tensor]], None]] = None,
+                               on_image: Optional[Callable[[int, torch.Tensor], None]] = None) -> Dict:
+        """One scene's rollout (gs_simulation.py:395-634): returns the per-frame render-space positions (and covariances when
+        the scene has them) unless `on_frame(frame, pos, cov)` consumes them. A scene with `shs` and `camera_params` is also
+        rendered each frame (the Gaussians only, from the frame's camera); the (3, H, W) images go to `on_image(frame, image)`
+        or to the record's `frames_rgb`."""
         dev = self.device
         mp, tp = dict(sc.material_params), sc.time_params
         n_grid, grid_lim = int(mp.get("n_grid", 64)), float(mp.get("grid_lim", 2.0))
@@ -178,23 +190,58 @@ class SceneBatchDriver:
                                                                   exact_box_semantics=False)
         substep_dt = tp["substep_dt"]
         step_per_frame = int(tp["frame_dt"] / substep_dt)                                           # float division like :627
-        frames_pos, frames_cov = [], []
+        frames_pos, frames_cov, frames_rgb = [], [], []
         filled = gs_num != int(pos0.shape[0])
+        render = self._render_setup(sc, rots, scale_origin, original_mean_pos, gs_num) if sc.shs is not None and sc.camera_params is not None \
+            else None
         for frame in range(int(tp["frame_num"])):
             pos = solver.export_particle_x_to_torch()
             cov = solver.export_particle_cov_to_torch().view(-1, 6) if sc.cov is not None else None
             if filled:                                                                             # the Gaussians only (:591, 594)
                 pos, cov = pos[:gs_num], cov[:gs_num]
             pr, cr = frame_export.render_frame_transform(pos, cov, sc.z_shift_value, scale_origin, original_mean_pos, rots)
+            if render is not None:
+                image = render(frame, pr, cr)
+                if on_image is not None:
+                    on_image(frame, image)
+                else:
+                    frames_rgb.append(image)
             if on_frame is not None:
                 on_frame(frame, pr, cr)
             else:
                 frames_pos.append(pr.clone())
                 frames_cov.append(None if cr is None else cr.clone())
             solver.p2g2p_n(step_per_frame, substep_dt)
-        return {"name": sc.name, "n_particles": int(pos0.shape[0]), "n_gaussians": gs_num, "frames_pos": frames_pos, "frames_cov": frames_cov,
-                "material_ids": props[4], "E": props[2], "substeps": step_per_frame * int(tp["frame_num"]), "time": solver.time,
-                "bc_conditions": bc_conditions}
+        record = {"name": sc.name, "n_particles": int(pos0.shape[0]), "n_gaussians": gs_num, "frames_pos": frames_pos, "frames_cov": frames_cov,
+                  "material_ids": props[4], "E": props[2], "substeps": step_per_frame * int(tp["frame_num"]), "time": solver.time,
+                  "bc_conditions": bc_conditions}
+        if render is not None:
+            record["frames_rgb"] = frames_rgb
+        return record
+
+    def _render_setup(self, sc: Scene, rots, scale_origin, original_mean_pos, gs_num: int):
+        """gs_simulation.py:529-540, 573-619: the view centre and orbit basis once, then per frame the camera for that frame
+        index and the Gaussians rasterised with their original opacity and SH (roll 0: the reference passes none)."""
+        if sc.cov is None or sc.opacity is None:
+            raise ValueError(f"scene {sc.name}: rendering needs the Gaussians' cov and opacity")
+        if sc.cameras is None:
+            raise ValueError(f"scene {sc.name}: rendering needs the model's cameras (the cameras.json list or its path)")
+        dev = self.device
+        shs = sc.shs.to(dev, torch.float32).contiguous()
+        opacity = sc.opacity.to(dev, torch.float32).reshape(-1).contiguous()
+        if shs.dim() != 3 or shs.shape[0] != gs_num or opacity.shape[0] != gs_num:
+            raise ValueError(f"scene {sc.name}: shs must be (N, K, 3) and opacity (N,) for the N = {gs_num} Gaussians")
+        cp = gs_render.decode_camera_params(sc.camera_params)
+        cams = gs_render.load_cameras(sc.cameras)
+        center, basis = gs_render.get_center_view_worldspace_and_observant_coordinate(
+            cp["mpm_space_viewpoint_center"], cp["mpm_space_vertical_upward_axis"], rots, scale_origin, original_mean_pos)
+        bg = [1.0, 1.0, 1.0] if sc.white_bg else [0.0, 0.0, 0.0]
+
+        def render(frame: int, pos: torch.Tensor, cov: torch.Tensor) -> torch.Tensor:
+            cam = gs_render.get_camera_view(cams, cp["default_camera_index"], center, basis, False, cp["init_azimuthm"], cp["init_elevation"],
+                                            cp["init_radius"], None, cp["move_camera"], frame, cp["delta_a"], cp["delta_e"], cp["delta_r"])
+            return gs_render.rasterize(pos, cov, opacity, cam, bg, shs=shs, sh_degree=sc.sh_degree)[0]
+        return render
 
     def _fill(self, sc: Scene, pos0: torch.Tensor, cov0: Optional[torch.Tensor], n_grid: int, grid_lim: float):
         """Particle filling of gs_simulation.py:442-462, 479-480: the Gaussians first, then the filled particles with
