@@ -83,7 +83,8 @@ int pixie_pack_predictions(const float* seg_logits_dev, const float* cont_dev, f
                            int64_t voxels, int n_classes, void* stream);
 /* ---- material field -> particles (SURVEY.md 8f-1). All array pointers are DEVICE pointers unless marked host.
  * pixie_field_extract: pixie/voxel/map_pred_to_coords.py:41-75 (unscale_prediction: clip to [-1,1], 10**log for density
- * and E, linear nu) + :198-245 (argmax material id, confidence = max class value, np.linspace voxel centres, mask > 0
+ * and E, linear nu) + :122-126, 198-245 (material id = argmax of the class channels, or the truncated class index when
+ * n_classes == 1 and D == 64; confidence = max class value, 1 for one channel; np.linspace voxel centres, mask > 0
  * compaction in C order). pred = packed (3 + n_classes, D, D, D) fp32, mask = (D, D, D) fp32. ranges (host) =
  * {density_min, density_max, E_min, E_max, nu_min, nu_max} of normalization_ranges.yaml. Outputs need room for D^3
  * entries; *count_host = number of occupied voxels. Synchronises `stream`. */
@@ -93,10 +94,11 @@ int pixie_field_extract(const float* pred_dev, int n_classes, const float* mask_
 /* pixie_knn_assign: PG/material_field.py:228-293 (perform_knn_smoothing) with assign_from_neighbors (:57-86): exact k nearest
  * material points per query (k <= 16), continuous properties = mean (np.mean order) or inverse-distance weighted mean,
  * categorical = mode (Counter.most_common / weighted bincount); queries farther than nn_distance_threshold from their nearest
- * point receive the defaults {density, E, nu, conf}, default_material, default_part. *n_too_far_host counts them. */
+ * point (compared in fp64, like scikit-learn's distances) receive the defaults {density, E, nu, conf}, default_material,
+ * default_part. *n_too_far_host counts them. k must not exceed n_points (scikit-learn raises there too). */
 int pixie_knn_assign(const float* query_dev, int n_query, const float* pos_dev, const float* density_dev, const float* E_dev,
                      const float* nu_dev, const int* material_dev, const int* part_dev, const float* conf_dev, int n_points, int k,
-                     float nn_distance_threshold, int weighted, const float defaults_host[4], int default_material, int default_part,
+                     double nn_distance_threshold, int weighted, const float defaults_host[4], int default_material, int default_part,
                      float* out_density_dev, float* out_E_dev, float* out_nu_dev, int* out_material_dev, int* out_part_dev,
                      float* out_conf_dev, int* n_too_far_host, void* stream);
 /* pixie_dbscan: the clustering of PG/material_field.py:365-480 (handle_stationary_clusters), scikit-learn DBSCAN semantics:

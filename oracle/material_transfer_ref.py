@@ -39,10 +39,11 @@ def unscale_prediction(pred_tensor: np.ndarray, r: dict) -> np.ndarray:
 
 def vertex_table(scaled_pred: np.ndarray, mask: np.ndarray, min_bounds, max_bounds, r: dict) -> dict:
     """The vertex records map_pred_to_ply writes (:198-245), as arrays: occupied voxels in C order, voxel centres from
-    np.linspace over the bounds (meshgrid 'ij'), id = argmax of the class channels, conf = their maximum."""
+    np.linspace over the bounds (meshgrid 'ij'), id = argmax of the class channels, conf = their maximum. A (1, 64, 64, 64)
+    class block holds the ids themselves (get_mat_id), truncated by the 'i4' fields, with conf = 1."""
     field = unscale_prediction(scaled_pred, r)
     classes = field[3:]
-    ids = classes[0] if classes.shape[0] == 1 else np.argmax(classes, axis=0)            # get_mat_id :122-126
+    ids = classes[0] if classes.shape == (1, 64, 64, 64) else np.argmax(classes, axis=0)  # get_mat_id :122-126
     axes = [np.linspace(min_bounds[d], max_bounds[d], mask.shape[d]) for d in range(3)]
     centres = np.stack(np.meshgrid(*axes, indexing="ij"), axis=-1)
     keep = mask > 0

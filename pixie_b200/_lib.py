@@ -7,7 +7,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpixie_b200.so")
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 
 class PixieError(RuntimeError):
@@ -87,7 +87,7 @@ _SIGNATURES = {
     "pixie_field_extract": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double),
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_void_p]),
     "pixie_knn_assign": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
-                                   C.c_int, C.c_float, C.c_int, C.POINTER(C.c_float), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_int, C.c_double, C.c_int, C.POINTER(C.c_float), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_void_p]),
     "pixie_dbscan": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int),
                                C.POINTER(C.c_int), C.c_void_p]),

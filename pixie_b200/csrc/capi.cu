@@ -24,7 +24,7 @@ struct pixie_gs_renderer_s { pixie::GsRenderer* r; };
 extern "C" {
 
 const char* pixie_last_error(void) { return g_err.c_str(); }
-int pixie_abi_version(void) { return 1; }
+int pixie_abi_version(void) { return 2; }
 
 int pixie_device_ok(void) {
     int dev = 0;
@@ -90,13 +90,14 @@ int pixie_field_extract(const float* pred, int n_classes, const float* mask, int
     return 0;
 }
 int pixie_knn_assign(const float* query, int nq, const float* pos, const float* density, const float* E, const float* nu, const int* material,
-                     const int* part, const float* conf, int m, int k, float threshold, int weighted, const float defaults[4], int def_material,
+                     const int* part, const float* conf, int m, int k, double threshold, int weighted, const float defaults[4], int def_material,
                      int def_part, float* o_density, float* o_E, float* o_nu, int* o_material, int* o_part, float* o_conf, int* n_too_far_host,
                      void* stream) {
     if (!query || !pos || !density || !E || !nu || !material || !part || !conf || !defaults || !o_density || !o_E || !o_nu || !o_material ||
         !o_part || !o_conf || !n_too_far_host) return set_err("null argument");
     if (k < 1 || k > 16) return set_err("knn_assign: k must be in [1, 16]");
     if (m < 1) return set_err("knn_assign: empty material point cloud");
+    if (k > m) return set_err("knn_assign: k exceeds the number of material points");
     if (require_device()) return 1;
     if (pixie::knn_assign(query, nq, pos, density, E, nu, material, part, conf, m, k, threshold, weighted, defaults, def_material, def_part,
                           o_density, o_E, o_nu, o_material, o_part, o_conf, n_too_far_host, (cudaStream_t)stream))
@@ -123,7 +124,8 @@ int pixie_cluster_stats(const float* pos, const int* index, const int* labels, i
     return 0;
 }
 int pixie_particle_volume(const float* pos, int n, int grid_n, float grid_dx, float* vol, void* stream) {
-    if (!pos || !vol) return set_err("null argument");
+    if (n < 0) return set_err("particle_volume: negative point count");
+    if (n > 0 && (!pos || !vol)) return set_err("null argument");
     if (grid_n < 1 || !(grid_dx > 0.f)) return set_err("particle_volume: bad grid");
     if (require_device()) return 1;
     if (pixie::particle_volume(pos, n, grid_n, grid_dx, vol, (cudaStream_t)stream)) return set_err("particle_volume failed");
@@ -131,7 +133,8 @@ int pixie_particle_volume(const float* pos, int n, int grid_n, float grid_dx, fl
 }
 int pixie_frame_transform(const float* pos, const float* cov, int n, float z_shift, float scale, const float mean[3], const float* rotations,
                           int n_rot, float* pos_out, float* cov_out, void* stream) {
-    if (!pos || !mean || !pos_out || (cov && !cov_out) || (n_rot > 0 && !rotations)) return set_err("null argument");
+    if (n < 0) return set_err("frame_transform: negative point count");
+    if (!mean || (n > 0 && (!pos || !pos_out || (cov && !cov_out))) || (n_rot > 0 && !rotations)) return set_err("null argument");
     if (n_rot < 0 || n_rot > 8) return set_err("frame_transform: at most 8 rotations");
     if (require_device()) return 1;
     if (pixie::frame_transform(pos, cov, n, z_shift, scale, mean, rotations, n_rot, pos_out, cov_out, (cudaStream_t)stream)) return set_err("frame_transform failed");

@@ -52,14 +52,20 @@ __global__ void field_extract_kernel(const ExtractArgs a) {
     a.density[o] = powf(10.f, dl);
     a.E[o] = powf(10.f, el);
     a.nu[o] = (c3[2] + 1.0f) * (float)((a.hi[2] - a.lo[2]) / 2.0) + (float)a.lo[2];
-    // get_mat_id: argmax over the class channels (first maximum); conf = that maximum
-    int best = 0;
+    // get_mat_id: a (1, 64, 64, 64) class block holds class indices, stored as 'i4' in the PLY (float -> int truncates);
+    // otherwise argmax over the class channels (first maximum), so a single channel of another size gives 0.
+    // conf = the maximum for K > 1, else 1
     float bv = a.pred[(size_t)3 * n + i];
-    for (int k = 1; k < a.K; ++k) {
-        const float v = a.pred[(size_t)(3 + k) * n + i];
-        if (v > bv) { bv = v; best = k; }
+    if (a.K == 1 && D == 64) {
+        a.material[o] = (int)bv;
+    } else {
+        int best = 0;
+        for (int k = 1; k < a.K; ++k) {
+            const float v = a.pred[(size_t)(3 + k) * n + i];
+            if (v > bv) { bv = v; best = k; }
+        }
+        a.material[o] = best;
     }
-    a.material[o] = best;
     a.conf[o] = a.K > 1 ? bv : 1.0f;
 }
 
@@ -277,7 +283,7 @@ int field_extract(const float* pred, int n_classes, const float* mask, int D, co
 }
 
 int knn_assign(const float* query, int nq, const float* pos, const float* density, const float* E, const float* nu, const int* material,
-               const int* part, const float* conf, int m, int k, float threshold, int weighted, const float defaults[4], int def_material,
+               const int* part, const float* conf, int m, int k, double threshold, int weighted, const float defaults[4], int def_material,
                int def_part, float* o_density, float* o_E, float* o_nu, int* o_material, int* o_part, float* o_conf, int* n_too_far_host,
                cudaStream_t st) {
     if (k < 1 || k > kKnnMaxK) return 2;
@@ -286,7 +292,7 @@ int knn_assign(const float* query, int nq, const float* pos, const float* densit
     cudaMemsetAsync(d_cnt, 0, sizeof(int), st);
     KnnArgs a{};
     a.query = query; a.nq = nq; a.pos = pos; a.density = density; a.E = E; a.nu = nu; a.conf = conf; a.material = material; a.part = part; a.m = m;
-    a.k = k; a.threshold = (double)threshold; a.weighted = weighted;
+    a.k = k; a.threshold = threshold; a.weighted = weighted;
     a.def_density = defaults[0]; a.def_E = defaults[1]; a.def_nu = defaults[2]; a.def_conf = defaults[3]; a.def_material = def_material; a.def_part = def_part;
     a.o_density = o_density; a.o_E = o_E; a.o_nu = o_nu; a.o_conf = o_conf; a.o_material = o_material; a.o_part = o_part; a.n_too_far = d_cnt;
     if (nq > 0) knn_assign_kernel<<<(nq + 127) / 128, 128, 0, st>>>(a);

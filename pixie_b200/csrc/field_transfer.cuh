@@ -13,7 +13,7 @@ int field_extract(const float* pred, int n_classes, const float* mask, int D, co
 // For every query point: k nearest material points -> mean (continuous) / mode (categorical) of their properties; queries whose
 // nearest point is farther than `threshold` get the defaults. defaults = {density, E, nu, conf}.
 int knn_assign(const float* query, int nq, const float* pos, const float* density, const float* E, const float* nu, const int* material,
-               const int* part, const float* conf, int m, int k, float threshold, int weighted, const float defaults[4], int def_material,
+               const int* part, const float* conf, int m, int k, double threshold, int weighted, const float defaults[4], int def_material,
                int def_part, float* o_density, float* o_E, float* o_nu, int* o_material, int* o_part, float* o_conf, int* n_too_far_host,
                cudaStream_t st);
 

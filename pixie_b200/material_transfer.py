@@ -83,11 +83,14 @@ def perform_knn_smoothing(query_positions: torch.Tensor, params: Dict[str, torch
     """material_field.py:228-293. `query_positions`: (Np, 3) MPM particle positions ALREADY in the material field's frame
     (the reference applies undoshift2center111 / undotransform2origin / inverse rotations first, :245-248 — elementwise torch).
     Returns (part_labels, densities, E_values, nu_values, material_ids, conf_values) like the reference."""
-    lib = _lib.require_device()
     n_particles = int(query_positions.shape[0])
     keys = ("part_labels", "density", "E", "nu", "material_id", "conf")
     if len(params["part_labels"]) == n_particles:                                   # :236-238 no smoothing needed
         return tuple(params[k] for k in keys)
+    m = int(params["pos"].shape[0])
+    if int(k_smoothing_neighbors) > m:                                              # NearestNeighbors.kneighbors raises here too
+        raise ValueError(f"Expected n_neighbors <= n_samples_fit, but n_neighbors = {k_smoothing_neighbors}, n_samples_fit = {m}")
+    lib = _lib.require_device()
     if not query_positions.is_cuda:
         raise _lib.PixieError("perform_knn_smoothing requires CUDA tensors; there is no CPU fallback")
     dev = query_positions.device
@@ -96,7 +99,6 @@ def perform_knn_smoothing(query_positions: torch.Tensor, params: Dict[str, torch
     q, pos = f(query_positions), f(params["pos"])
     dens, E, nu, conf = f(params["density"]), f(params["E"]), f(params["nu"]), f(params["conf"])
     mat, part = i(params["material_id"]), i(params["part_labels"])
-    m = int(pos.shape[0])
     # get_defaults (:38-50): mean of each continuous property, "stationary" material, part label 0
     mean = lambda t, key: float(t.mean().item()) if m > 0 else float(DEFAULT_VALUES.get(key, 0.0))
     defaults = (C.c_float * 4)(mean(dens, "density"), mean(E, "E"), mean(nu, "nu"), mean(conf, "conf"))

@@ -204,6 +204,25 @@ def main():
         blob[f"field/table/{k}"] = np.asarray(tab[k]).copy()
     print("map_pred_to_ply:", len(tab), "vertices; ids", np.unique(tab["material_id"], return_counts=True))
 
+    # ---------------------------------------------------------------- f-1a': a label-map prediction, (3 + 1, 64, 64, 64):
+    # get_mat_id returns the class channel itself and the 'i4' PLY fields truncate it (own RNG: the arrays above are unchanged)
+    irng = np.random.default_rng(17)
+    iidx, ivals = field_inputs(seed=6)
+    ivals = np.concatenate([ivals[:, :3], irng.integers(0, 8, size=(len(iidx), 1)).astype(np.float32)], axis=1)
+    odd = irng.choice(len(iidx), size=60, replace=False)
+    ivals[odd, 3] = irng.choice(np.array([2.75, -0.5, 7.999, 0.25, 5.5], np.float32), size=60)
+    ipred, imask = dense(iidx, ivals)
+    with tempfile.TemporaryDirectory() as td:
+        np.save(td + "/pred.npy", ipred)
+        np.save(td + "/mask.npy", imask)
+        np.savez(td + "/grid.npz", min_bounds=lo, max_bounds=hi, grid_shape=np.array([64, 64, 64]))
+        ns["map_pred_to_ply"](td + "/pred.npy", td + "/mask.npy", td + "/grid.npz", td + "/out.ply", "obj", cfg=cfg)
+    itab = _Capture.table
+    blob.update({"field_index/idx": iidx, "field_index/vals": ivals})
+    for k in ("x", "y", "z", "part_label", "density", "E", "nu", "material_id", "conf"):
+        blob[f"field_index/table/{k}"] = np.asarray(itab[k]).copy()
+    print("map_pred_to_ply (class indices):", len(itab), "vertices; ids", np.unique(itab["material_id"], return_counts=True))
+
     # ---------------------------------------------------------------- f-1b: perform_knn_smoothing
     tns = {"torch": _TorchCPU(), "np": np}
     extract(PG + "/utils/transformation_utils.py",
