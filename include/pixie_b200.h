@@ -155,7 +155,10 @@ int pixie_fill_grids(int* count_dev, const float* density_dev, int grid_n, float
  * stores them (16 floats each, row-vector convention). image_dev [3][height][width] receives the unclamped RGB image over
  * bg, radii_dev [n] the screen radius (0 = culled). The call synchronises `stream` once, for the number of (Gaussian, tile)
  * pairs, which goes to *n_rendered_host (may be NULL). phase_ms_host, when not NULL, receives the times in ms of preprocess,
- * scan + keys, sort, ranges and blend (CUDA events; the call then synchronises a second time). */
+ * scan + keys, sort, ranges and blend (CUDA events; the call then synchronises a second time). The frame returns with its
+ * sort and blend still running on `stream`; the next frame of the same renderer, on any stream, first waits for them, so
+ * frames run in call order whatever streams they are drawn on. A renderer is not safe to call from two host threads at
+ * once: callers serialise its calls. */
 typedef struct pixie_gs_renderer_s* pixie_gs_renderer_t;
 int pixie_gs_renderer_create(pixie_gs_renderer_t* out);
 int pixie_gs_render(pixie_gs_renderer_t h, const float* means_dev, const float* cov_dev, const float* opacity_dev,

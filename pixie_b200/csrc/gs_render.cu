@@ -12,6 +12,10 @@
 //               shared memory with cp.async: batch b+1 is in flight while batch b blends. The CTA leaves at the first
 //               batch boundary where every pixel has saturated.
 //
+// A renderer's buffers serve every frame it draws, and a frame returns once its blend is enqueued. So each frame's stream
+// first waits for the event the previous frame recorded after its blend: frames drawn on different streams run one after
+// another, in call order, and a frame on the same stream pays nothing for it.
+//
 // The per-Gaussian arithmetic follows the reference's operation order (glm's column-major products, the double-precision
 // pixel mapping) so radii and composited sets agree with it; see DESIGN.md §7.
 #include "gs_render.cuh"
@@ -277,6 +281,7 @@ struct GsRenderer {
     void* tmp = nullptr;
     unsigned long long* total_host = nullptr;   // pinned
     cudaEvent_t ev[6] = {};
+    cudaEvent_t last = nullptr;                  // recorded after each frame's last kernel; the next frame waits for it
 };
 
 namespace {
@@ -305,6 +310,7 @@ GsRenderer* gs_renderer_create() {
     if (cudaMallocHost(&r->total_host, sizeof(unsigned long long)) != cudaSuccess) { delete r; return nullptr; }
     for (auto& e : r->ev)
         if (cudaEventCreate(&e) != cudaSuccess) { gs_renderer_destroy(r); return nullptr; }
+    if (cudaEventCreateWithFlags(&r->last, cudaEventDisableTiming) != cudaSuccess) { gs_renderer_destroy(r); return nullptr; }
     return r;
 }
 
@@ -316,12 +322,15 @@ void gs_renderer_destroy(GsRenderer* r) {
     if (r->total_host) cudaFreeHost(r->total_host);
     for (auto& e : r->ev)
         if (e) cudaEventDestroy(e);
+    if (r->last) cudaEventDestroy(r->last);
     delete r;
 }
 
 const char* gs_error(GsRenderer* r) { return r->err.c_str(); }
 
-int gs_render(GsRenderer* r, const GsRenderArgs& a, int* n_rendered, float* phase_ms, cudaStream_t st) {
+namespace {
+
+int render_frame(GsRenderer* r, const GsRenderArgs& a, int* n_rendered, float* phase_ms, cudaStream_t st) {
     const int n = a.n;
     Cam c;
     for (int k = 0; k < 16; ++k) { c.view[k] = a.view[k]; c.proj[k] = a.proj[k]; }
@@ -407,6 +416,16 @@ int gs_render(GsRenderer* r, const GsRenderArgs& a, int* n_rendered, float* phas
     }
     if (n_rendered) *n_rendered = L;
     return 0;
+}
+
+}  // namespace
+
+int gs_render(GsRenderer* r, const GsRenderArgs& a, int* n_rendered, float* phase_ms, cudaStream_t st) {
+    if (cudaStreamWaitEvent(st, r->last, 0) != cudaSuccess) return fail(r, "gs_render: waiting for the previous frame");
+    const int rc = render_frame(r, a, n_rendered, phase_ms, st);
+    // recorded on failure too: whatever the frame enqueued before failing still reads and writes the shared buffers
+    if (cudaEventRecord(r->last, st) != cudaSuccess && rc == 0) return fail(r, "gs_render: recording the frame's end");
+    return rc;
 }
 
 }  // namespace pixie

@@ -25,7 +25,8 @@ GsRenderer* gs_renderer_create();
 void gs_renderer_destroy(GsRenderer* r);
 // One frame on `st`. Synchronises `st` once, for the number of (Gaussian, tile) pairs. *n_rendered receives it. With
 // phase_ms non-NULL, also records events between the phases and writes their times (preprocess, scan + keys, sort,
-// ranges, blend; a second synchronise). Returns 0, or non-zero with gs_error(r) set.
+// ranges, blend; a second synchronise). Returns 0, or non-zero with gs_error(r) set. `st` first waits for the end of
+// the renderer's previous frame, so frames on different streams run in call order. One host thread at a time per renderer.
 int gs_render(GsRenderer* r, const GsRenderArgs& a, int* n_rendered, float* phase_ms, cudaStream_t st);
 const char* gs_error(GsRenderer* r);
 

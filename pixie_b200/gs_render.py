@@ -10,7 +10,9 @@ The camera arithmetic runs in float64 numpy and is cast to float32 where the ref
 float32, the projection matrix is a float32 tensor); the view centre is computed in float64 where the reference
 computes it in float32. Colours from `shs` are evaluated toward the camera centre inside the rasterizer's preprocess
 kernel as convert_SH (utils/render_utils.py:113-130) does: +0.5, clamped at 0. The image is RGB, float32, unclamped.
-The forward pass only; no CPU fallback. Work runs on the current stream of the tensors' device.
+The forward pass only; no CPU fallback. Work runs on the current stream of the tensors' device. One renderer per
+device serves every call: a frame waits on the device for the previous one, whatever stream either is drawn on, and
+calls from several host threads take turns.
 """
 from __future__ import annotations
 
@@ -18,6 +20,7 @@ import ctypes as C
 import json
 import math
 import os
+import threading
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple, Union
 
@@ -229,10 +232,12 @@ def decode_camera_params(sim_params: Dict) -> Dict:
 
 # ------------------------------------------------------------------------------------------------ rasterizer
 _RENDERERS: Dict[int, "_Renderer"] = {}
+_RENDERERS_LOCK = threading.Lock()
 
 
 class _Renderer:
-    """One device's renderer handle; its buffers grow to the largest frame seen and are reused."""
+    """One device's renderer handle; its buffers grow to the largest frame seen and are reused. Its host-side state
+    (capacities, the pinned pair-count word, the error string) is guarded by `lock`."""
 
     def __init__(self, device: torch.device):
         lib = _lib.require_device()
@@ -240,6 +245,7 @@ class _Renderer:
         with torch.cuda.device(device):
             _lib.check(lib.pixie_gs_renderer_create(C.byref(h)))
         self.h, self.lib = h, lib
+        self.lock = threading.Lock()
 
     def __del__(self):
         if getattr(self, "h", None) and self.h.value:
@@ -248,9 +254,10 @@ class _Renderer:
 
 def _renderer(device: torch.device) -> _Renderer:
     idx = device.index if device.index is not None else torch.cuda.current_device()
-    if idx not in _RENDERERS:
-        _RENDERERS[idx] = _Renderer(torch.device("cuda", idx))
-    return _RENDERERS[idx]
+    with _RENDERERS_LOCK:
+        if idx not in _RENDERERS:
+            _RENDERERS[idx] = _Renderer(torch.device("cuda", idx))
+        return _RENDERERS[idx]
 
 
 def _f32(values, n: int, name: str):
@@ -299,7 +306,7 @@ def _rasterize(means3D, cov3D, opacity, camera: Camera, bg, shs=None, sh_degree:
     r = _renderer(dev)
     n_rendered = C.c_int(0)
     ms = (C.c_float * 5)() if phase_ms is not None else None
-    with torch.cuda.device(dev):
+    with torch.cuda.device(dev), r.lock:
         image = torch.empty((3, H, W), dtype=torch.float32, device=dev)
         radii = torch.empty((n,), dtype=torch.int32, device=dev)
         _lib.check(r.lib.pixie_gs_render(
