@@ -1,6 +1,6 @@
 """Vectorised numpy restatement of the reference's particle filling (PG/particle_filling/filling.py:26-380, Taichi f32 / i32),
-fast enough for inputs of config size. Pinned to the reference's own kernels through tests/golden/filling_golden.npz
-(tests/golden/make_filling_golden.py executes them).
+fast enough for inputs of config size. Pinned to the reference's own kernels through tests/golden/filling_golden.npz and
+tests/golden/filling_edges_golden.npz (tests/golden/make_filling_golden.py and make_filling_edges_golden.py execute them).
 
 Float32 throughout like Taichi's default precision, with the reference's operation order inside one Gaussian's
 contribution; contributions are accumulated in a different order (np.add.at over groups of equal window radius), so
@@ -36,22 +36,25 @@ def densify_grids(pos, opacity, cov, grid_n, grid_dx, chunk=1 << 16):
     n, dx = int(grid_n), F32(grid_dx)
     count = np.zeros((n, n, n), np.int32)
     density = np.zeros(n ** 3, F32)
-    c0 = np.floor(pos / dx).astype(np.int64)
+    cap = 2.0 ** 40                                                                # |cell| and r: wider than any grid, no int64 overflow
+    c0 = np.clip(np.floor(pos / dx), -cap, cap).astype(np.int64)
     cc = np.clip(c0, 0, n - 1)
     np.add.at(count, (cc[:, 0], cc[:, 1], cc[:, 2]), 1)
     sig, P = _sym_precision(cov)
-    r = np.minimum(np.ceil(np.sqrt(sig).max(axis=1) / dx), n).astype(np.int64)
+    r = np.minimum(np.ceil(np.sqrt(sig).max(axis=1) / dx), cap).astype(np.int64)
+    # the reference's window [c0 - r, c0 + r] clipped to the grid (clipping r instead loses cells of off-grid Gaussians)
+    lo = np.clip(c0 - r[:, None], 0, n)
+    size = np.clip(c0 + r[:, None], -1, n - 1) - lo + 1
+    live = np.all(size > 0, axis=1)
     corners = [(a, b, c) for a in range(2) for b in range(2) for c in range(2)]
-    for rv in np.unique(r):
-        ax = np.arange(-rv, rv + 1)
-        off = np.stack(np.meshgrid(ax, ax, ax, indexing="ij"), axis=-1).reshape(-1, 3)
-        sel = np.nonzero(r == rv)[0]
+    for shape in np.unique(size[live], axis=0):
+        off = np.stack(np.meshgrid(*[np.arange(s) for s in shape], indexing="ij"), axis=-1).reshape(-1, 3)
+        sel = np.nonzero(live & np.all(size == shape, axis=1))[0]
         for s in range(0, len(sel), max(1, chunk // len(off))):
             g = sel[s:s + max(1, chunk // len(off))]
-            cell = c0[g][:, None, :] + off[None]                                   # (G, W, 3)
-            ok = np.all((cell >= 0) & (cell < n), axis=-1)
+            cell = lo[g][:, None, :] + off[None]                                   # (G, W, 3)
             p, Pg = pos[g][:, None, :], P[g][:, None]
-            gw = np.zeros(ok.shape, F32)
+            gw = np.zeros(cell.shape[:2], F32)
             for corner in corners:
                 d = p - (cell + np.array(corner)).astype(F32) * dx
                 y = [(Pg[..., q, 0] * d[..., 0] + Pg[..., q, 1] * d[..., 1]) + Pg[..., q, 2] * d[..., 2] for q in range(3)]
@@ -59,7 +62,7 @@ def densify_grids(pos, opacity, cov, grid_n, grid_dx, chunk=1 << 16):
                 gw = gw + np.exp(F32(-0.5) * e)
             val = opacity[g][:, None] * gw / F32(8.0)
             flat = (cell[..., 0] * n + cell[..., 1]) * n + cell[..., 2]
-            np.add.at(density, flat[ok], val[ok])
+            np.add.at(density, flat.ravel(), val.ravel())
     return count, density.reshape(n, n, n)
 
 

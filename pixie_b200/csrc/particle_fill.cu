@@ -64,9 +64,13 @@ __device__ void sym_eig3(const float c[6], double w[3], double V[3][3]) {
             }
 }
 
+// Cells are held in 64 bits, and |cell| and the window radius are capped at 2^40 cells (far wider than any grid), so that
+// a Gaussian at |p / dx| ~ 1e30 gets an empty window instead of wrapping around.
+__device__ __forceinline__ long long cap_cells(float x) { return (long long)fminf(fmaxf(x, -0x1p40f), 0x1p40f); }
+
 // Gaussians per cell with the clamp of get_particle_volume (the reference indexes out of range for a Gaussian outside the
-// grid); the splat window below uses the unclamped cell with the reference's per-cell bounds test.
-__device__ __forceinline__ int clamp_cell(int i, int n) { return min(max(i, 0), n - 1); }
+// grid); the splat window below is the reference's window around the unclamped cell, clipped to the grid.
+__device__ __forceinline__ int clamp_cell(long long i, int n) { return (int)min(max(i, 0ll), (long long)n - 1); }
 
 __global__ void __launch_bounds__(128)
 fill_density_kernel(const float* __restrict__ pos, const float* __restrict__ opacity, const float* __restrict__ cov, int n,
@@ -74,9 +78,9 @@ fill_density_kernel(const float* __restrict__ pos, const float* __restrict__ opa
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= n) return;
     const float p[3] = {pos[3 * g], pos[3 * g + 1], pos[3 * g + 2]};
-    int c0[3];
+    long long c0[3];
 #pragma unroll
-    for (int d = 0; d < 3; ++d) c0[d] = (int)floorf(__fdiv_rn(p[d], dx));   // ti.floor(x / grid_dx, dtype=int), IEEE f32
+    for (int d = 0; d < 3; ++d) c0[d] = cap_cells(floorf(__fdiv_rn(p[d], dx)));   // ti.floor(x / grid_dx, dtype=int), IEEE f32
     atomicAdd(count + ((size_t)clamp_cell(c0[0], gn) * gn + clamp_cell(c0[1], gn)) * gn + clamp_cell(c0[2], gn), 1);
 
     float cv[6];
@@ -104,16 +108,19 @@ fill_density_kernel(const float* __restrict__ pos, const float* __restrict__ opa
     float rr = 0.0f;
 #pragma unroll
     for (int k = 0; k < 3; ++k) rr = fmaxf(rr, sqrtf(sig[k]));
-    // r = ceil(max sqrt(sig) / dx); a window wider than the grid is clipped by the bounds test anyway
-    const int r = (int)fminf(ceilf(__fdiv_rn(rr, dx)), (float)gn);
+    // r = ceil(max sqrt(sig) / dx). The window [c0 - r, c0 + r] is clipped to the grid, not r: a Gaussian whose cell lies
+    // outside the grid can still reach across all of it. An empty window becomes lo = gn or hi = -1, both safe as int.
+    const long long r = cap_cells(ceilf(__fdiv_rn(rr, dx)));
     const float op = opacity[g];
-    const int lo0 = max(-r, -c0[0]), hi0 = min(r, gn - 1 - c0[0]);
-    const int lo1 = max(-r, -c0[1]), hi1 = min(r, gn - 1 - c0[1]);
-    const int lo2 = max(-r, -c0[2]), hi2 = min(r, gn - 1 - c0[2]);
-    for (int a = lo0; a <= hi0; ++a)
-        for (int b = lo1; b <= hi1; ++b)
-            for (int c = lo2; c <= hi2; ++c) {
-                const int ci = c0[0] + a, cj = c0[1] + b, ck = c0[2] + c;
+    int lo[3], hi[3];
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+        lo[d] = (int)min(max(c0[d] - r, 0ll), (long long)gn);
+        hi[d] = (int)max(min(c0[d] + r, (long long)gn - 1), -1ll);
+    }
+    for (int ci = lo[0]; ci <= hi[0]; ++ci)
+        for (int cj = lo[1]; cj <= hi[1]; ++cj)
+            for (int ck = lo[2]; ck <= hi[2]; ++ck) {
                 float gw = 0.0f;                      // compute_density (:13-23): 8 corners in i, j, k order
 #pragma unroll
                 for (int u = 0; u < 2; ++u)

@@ -1,6 +1,6 @@
 """A serial float32 / int32 stand-in for the part of `taichi` that PG/particle_filling/filling.py uses, so that its kernels
 (densify_grids, fill_dense_grids, collision_search, collision_times, internal_filling, fill_particles) can be exec'd as they
-are written. Used by make_filling_golden.py only.
+are written. Used by make_filling_golden.py and make_filling_edges_golden.py only.
 
 Arithmetic follows Taichi's default precision: every float is float32 (Python float literals and `float` kernel arguments
 are rounded to float32 first), every int int32, and vector / matrix products are summed left to right in float32, one
@@ -99,28 +99,40 @@ class Matrix:
 
 
 class Field:
-    def __init__(self, dtype, shape, n=None):
+    """Every access is bounds-checked. `lenient=True` (int scalar fields only, opt-in) instead drops out-of-range writes and
+    reads them as 0: the count write of a Gaussian outside the grid, which is an undefined out-of-range store in Taichi."""
+
+    def __init__(self, dtype, shape, n=None, lenient=False):
         shp = (shape,) if np.isscalar(shape) else tuple(shape)
+        assert not lenient or (dtype is int and not n), "lenient access is for int scalar fields only"
         self.a = np.zeros(shp + ((n,) if n else ()), F32 if dtype is float else I32)
-        self.shape, self.n = shp, n
+        self.shape, self.n, self.lenient = shp, n, lenient
 
     def _key(self, idx):
         if isinstance(idx, Vector):
             idx = idx.idx()
         if isinstance(idx, tuple):
             idx = tuple(int(i) for i in idx)
-            assert all(0 <= i < s for i, s in zip(idx, self.shape)), ("out-of-range field access", idx, self.shape)
+            ok = all(0 <= i < s for i, s in zip(idx, self.shape))
         else:
             idx = int(idx)
-            assert 0 <= idx < self.shape[0], ("out-of-range field access", idx, self.shape)
+            ok = 0 <= idx < self.shape[0]
+        if not ok and self.lenient:
+            return None
+        assert ok, ("out-of-range field access", idx, self.shape)
         return idx
 
     def __getitem__(self, idx):
-        x = self.a[self._key(idx)]
+        key = self._key(idx)
+        if key is None:
+            return 0
+        x = self.a[key]
         return Vector(list(x)) if self.n else _scalar(x)
 
     def __setitem__(self, idx, v):
-        self.a[self._key(idx)] = list(v) if isinstance(v, Vector) else v
+        key = self._key(idx)
+        if key is not None:
+            self.a[key] = list(v) if isinstance(v, Vector) else v
 
     def __iter__(self):                      # struct-for over the field's cells, C order
         return iter(np.ndindex(*self.shape))
