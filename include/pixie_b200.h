@@ -145,6 +145,12 @@ int pixie_fill_density(const float* pos_dev, const float* opacity_dev, const flo
 int pixie_fill_grids(int* count_dev, const float* density_dev, int grid_n, float grid_dx, const float origin_host[3],
                      float density_thres, float search_thres, int max_particles_per_cell, int exclude_dir, int ray_cast_dir,
                      unsigned long long seed, float* out_dev, int max_samples, int* n_dense_host, int* n_total_host, void* stream);
+/* pixie_nearest_gaussian: the search of get_attr_from_closest (filling.py:383-405). index_dev[j] = the i minimising the
+ * float32 distance d = sqrt((dx*dx + dy*dy) + dz*dz), dx = query[j].x - pos[i].x (one rounding per operation), ties to the
+ * lowest i; -1 when no Gaussian has d < 1e10 (n = 0, a non-finite query, or all Gaussians that far). Exact, through a
+ * bounding-volume tree (not O(m n)). pos_dev [n][3], query_dev [m][3], index_dev [m] int32; n or m may be 0. Stream-ordered,
+ * no host sync; repeat calls give identical results. */
+int pixie_nearest_gaussian(const float* pos_dev, int n, const float* query_dev, int m, int* index_dev, void* stream);
 /* ---- Gaussian-splatting rasteriser, forward only (gs_simulation.py:573-631 with `--render_img`: Inria's
  * diff-gaussian-rasterization at scale_modifier 1, prefiltered false, precomputed 3D covariances).
  * A renderer keeps its device buffers between frames and grows them when a frame needs more; once warm, a frame allocates

@@ -98,6 +98,7 @@ _SIGNATURES = {
     "pixie_fill_density": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pixie_fill_grids": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_float), C.c_float, C.c_float, C.c_int, C.c_int,
                                    C.c_int, C.c_ulonglong, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
+    "pixie_nearest_gaussian": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "pixie_gs_renderer_create": (C.c_int, [C.POINTER(C.c_void_p)]),
     "pixie_gs_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                   C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float, C.c_float, C.c_int, C.c_int,

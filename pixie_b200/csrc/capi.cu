@@ -6,6 +6,7 @@
 #include "field_transfer.cuh"
 #include "cluster.cuh"
 #include "particle_fill.cuh"
+#include "nearest.cuh"
 #include "gs_render.cuh"
 
 #include <algorithm>
@@ -166,6 +167,13 @@ int pixie_fill_grids(int* count, const float* density, int grid_n, float grid_dx
         return set_err("fill_grids: filling adds " + std::to_string(*n_total_host) + " particles (" + std::to_string(*n_dense_host) +
                        " in dense cells) but max_samples is " + std::to_string(max_samples));
     if (rc) return set_err("fill_grids failed");
+    return 0;
+}
+int pixie_nearest_gaussian(const float* pos, int n, const float* query, int m, int* index, void* stream) {
+    if (n < 0 || m < 0) return set_err("nearest_gaussian: negative count");
+    if ((n > 0 && m > 0 && !pos) || (m > 0 && (!query || !index))) return set_err("null argument");
+    if (require_device()) return 1;
+    if (pixie::nearest_gaussian(pos, n, query, m, index, (cudaStream_t)stream)) return set_err("nearest_gaussian failed");
     return 0;
 }
 // ------------------------------------------------------------------------------------- Gaussian rasteriser

@@ -7,11 +7,16 @@ enclose, with the reference's names, arguments and defaults:
     fill_particles(pos, opacity, cov, grid_n, max_samples, grid_dx, density_thres=2.0, search_thres=1.0,
                    max_particles_per_cell=1, search_exclude_dir=5, ray_cast_dir=4, boundary=None, smooth=False, seed=0)
     decode_filling_params(filling, material_params)          utils/decode_param.py:177-208 (defaults of the config block)
+    init_filled_particles(pos, shs, cov, opacity, new_pos)   filling.py:383-446 (`visualize`: each new particle takes the
+                                                             SH, opacity and covariance of its nearest Gaussian)
 
 Deviations from the reference: new particles come in a fixed order (dense cells first, then interior cells, each in C order
 of cells) with offsets drawn from a counter-based generator keyed on `seed`; a total above `max_samples` raises instead of
 writing out of bounds; a Gaussian outside the grid counts in the nearest border cell; `smooth` (PyMCubes constrained
-smoothing) is not available. No CPU fallback.
+smoothing) is not available. `init_filled_particles` finds the same nearest Gaussian as the reference's brute-force loop
+(same float32 distance, ties to the lowest index) through a tree instead of O(M N) work; where the reference would read
+index -1 (no Gaussian closer than 1e10: none at all, a NaN query, or all that far) it raises; with no new particles it
+returns its inputs. No CPU fallback.
 """
 from __future__ import annotations
 
@@ -144,3 +149,54 @@ def fill_particles(pos: torch.Tensor, opacity: torch.Tensor, cov: torch.Tensor, 
     new, _ = fill_grids(count, density, grid_dx, max_samples, density_thres, search_thres, max_particles_per_cell, search_exclude_dir,
                         ray_cast_dir, origin, seed)
     return torch.cat([pos_clone, new], dim=0)
+
+
+def nearest_gaussian(pos: torch.Tensor, query: torch.Tensor) -> torch.Tensor:
+    """The search of get_attr_from_closest (filling.py:383-405): (M,) int32, for each query the index of the Gaussian at
+    the smallest float32 distance (ties to the lowest index), or -1 when none is closer than 1e10. Exact, on the device."""
+    lib = _lib.require_device()
+    if not (pos.is_cuda and query.is_cuda):
+        raise _lib.PixieError("nearest_gaussian requires CUDA tensors; there is no CPU fallback")
+    if pos.dim() != 2 or pos.shape[1] != 3 or query.dim() != 2 or query.shape[1] != 3:
+        raise ValueError(f"pos and query must be (N, 3) and (M, 3), got {tuple(pos.shape)} and {tuple(query.shape)}")
+    dev = query.device
+    p = pos.detach().to(dev, torch.float32).contiguous()
+    q = query.detach().to(torch.float32).contiguous()
+    with torch.cuda.device(dev):
+        index = torch.empty(q.shape[0], dtype=torch.int32, device=dev)
+        _lib.check(lib.pixie_nearest_gaussian(C.c_void_p(p.data_ptr()), p.shape[0], C.c_void_p(q.data_ptr()), q.shape[0],
+                                              C.c_void_p(index.data_ptr()), _stream(dev)))
+    return index
+
+
+def init_filled_particles(pos: torch.Tensor, shs: torch.Tensor, cov: torch.Tensor, opacity: torch.Tensor,
+                          new_pos: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """init_filled_particles (filling.py:408-446), the `particle_filling.visualize` step: every new particle takes the SH,
+    opacity and covariance of its nearest Gaussian. pos (N, 3), shs (N, K, 3) with K in 1, 4, 9, 16, cov (N, 6), opacity
+    (N, 1) or (N,), new_pos (M, 3); returns (shs (N+M, K, 3), opacity (N+M, 1), cov (N+M, 6)) float32 on pos's device, the
+    Gaussians' rows first, then the copied rows bit for bit. Raises PixieError when a new particle has no Gaussian closer
+    than 1e10 (the reference would read index -1). With M = 0 the inputs come back in those shapes."""
+    if pos.dim() != 2 or pos.shape[1] != 3:
+        raise ValueError(f"pos must be (N, 3), got {tuple(pos.shape)}")
+    n = pos.shape[0]
+    if shs.dim() != 3 or shs.shape[0] != n or shs.shape[1] not in (1, 4, 9, 16) or shs.shape[2] != 3:
+        raise ValueError(f"shs must be (N, K, 3) with K in 1, 4, 9, 16 for N = {n} Gaussians, got {tuple(shs.shape)}")
+    if opacity.numel() != n or cov.numel() != 6 * n:
+        raise ValueError(f"opacity must hold N and cov N x 6 values for N = {n} Gaussians, got {tuple(opacity.shape)} and {tuple(cov.shape)}")
+    if new_pos.dim() != 2 or new_pos.shape[1] != 3:
+        raise ValueError(f"new_pos must be (M, 3), got {tuple(new_pos.shape)}")
+    if not (pos.is_cuda and shs.is_cuda and cov.is_cuda and opacity.is_cuda and new_pos.is_cuda):
+        raise _lib.PixieError("init_filled_particles requires CUDA tensors; there is no CPU fallback")
+    dev = pos.device
+    s = shs.detach().to(dev, torch.float32)
+    o = opacity.detach().to(dev, torch.float32).reshape(n, 1)
+    c = cov.detach().to(dev, torch.float32).reshape(n, 6)
+    if new_pos.shape[0] == 0:
+        return s.clone(), o.clone(), c.clone()
+    index = nearest_gaussian(pos, new_pos.to(dev))
+    missing = int((index < 0).sum())
+    if missing:
+        raise _lib.PixieError(f"init_filled_particles: {missing} of {index.shape[0]} new particles have no Gaussian closer than 1e10")
+    idx = index.long()
+    return (torch.cat([s, torch.index_select(s, 0, idx)]), torch.cat([o, torch.index_select(o, 0, idx)]),
+            torch.cat([c, torch.index_select(c, 0, idx)]))

@@ -60,6 +60,9 @@ class Scene:
     opacity: Optional[torch.Tensor] = None         # (N,) or (N, 1) opacities; needed by particle filling
     # the config's `particle_filling` block (decode_param.py:177-208 defaults applied here); None simulates the Gaussians only
     particle_filling: Optional[Dict] = None
+    # preprocessing_params["sim_area"] (gs_simulation.py:419-434): [x0, x1, y0, y1, z0, z1] in the rotated frame. Only the
+    # Gaussians strictly inside are simulated; the others are drawn unchanged in every rendered frame. None simulates all.
+    sim_area: Optional[Sequence[float]] = None
     # rendering (gs_simulation.py --render_img): with both `shs` and `camera_params`, every frame is rendered from the
     # scene's own opacity and SH coefficients; otherwise nothing is rendered
     shs: Optional[torch.Tensor] = None             # (N, 16, 3) SH coefficients, as GaussianModel.get_features
@@ -152,25 +155,52 @@ class SceneBatchDriver:
         """One scene's rollout (gs_simulation.py:395-634): returns the per-frame render-space positions (and covariances when
         the scene has them) unless `on_frame(frame, pos, cov)` consumes them. A scene with `shs` and `camera_params` is also
         rendered each frame (the Gaussians only, from the frame's camera); the (3, H, W) images go to `on_image(frame, image)`
-        or to the record's `frames_rgb`."""
+        or to the record's `frames_rgb`. With `sim_area`, only the Gaussians inside it are simulated and exported; the others
+        are appended, unchanged, to every rendered frame. With the filling block's `visualize`, the filled particles carry
+        their nearest Gaussian's SH, opacity and covariance and are exported and rendered like Gaussians."""
         dev = self.device
         mp, tp = dict(sc.material_params), sc.time_params
         n_grid, grid_lim = int(mp.get("n_grid", 64)), float(mp.get("grid_lim", 2.0))
         rots = [r.to(dev, torch.float32) for r in sc.rotation_matrices]
-        rotated = apply_rotations(sc.particles.to(dev, torch.float32), rots)
+        init_pos = sc.particles.to(dev, torch.float32)
+        rotated = apply_rotations(init_pos, rots)
+        init_cov = None if sc.cov is None else sc.cov.to(dev, torch.float32)
+        init_opacity = None if sc.opacity is None else sc.opacity.to(dev, torch.float32)
+        init_shs = None if sc.shs is None else sc.shs.to(dev, torch.float32)
+        unselected = None
+        if sc.sim_area is not None:
+            # gs_simulation.py:419-434: the Gaussians strictly inside the box (float32 positions against float32 bounds, as
+            # torch compares them) are simulated; the others keep their original frame, opacity and SH for rendering
+            b = [float(v) for v in sc.sim_area]
+            if len(b) != 6:
+                raise ValueError(f"scene {sc.name}: sim_area must be [x0, x1, y0, y1, z0, z1]")
+            mask = torch.ones(rotated.shape[0], dtype=torch.bool, device=dev)
+            for i in range(3):
+                mask &= (rotated[:, i] > b[2 * i]) & (rotated[:, i] < b[2 * i + 1])
+            if not bool(mask.any()):
+                raise ValueError(f"scene {sc.name}: no Gaussian lies strictly inside sim_area {b}")
+            keep = lambda t: None if t is None else t[mask]                                # noqa: E731
+            drop = lambda t: None if t is None else t[~mask]                               # noqa: E731
+            unselected = {"pos": drop(init_pos), "cov": drop(init_cov), "opacity": drop(init_opacity), "shs": drop(init_shs)}
+            rotated, init_cov, init_opacity, init_shs = rotated[mask], keep(init_cov), keep(init_opacity), keep(init_shs)
         transformed, scale_origin, original_mean_pos = transform2origin(rotated)
         pos0 = transformed + torch.tensor([1.0, 1.0, 1.0 + sc.z_shift_value], device=dev)          # shift2center111 :103-105
         cov0 = None
-        if sc.cov is not None:
+        if init_cov is not None:
             # apply_cov_rotations(init_cov, R) * scale^2  (gs_simulation.py:438): R C R^T per rotation, on the device
-            c = sc.cov.to(dev, torch.float32)
+            c = init_cov
             m = torch.stack([c[:, 0], c[:, 1], c[:, 2], c[:, 1], c[:, 3], c[:, 4], c[:, 2], c[:, 4], c[:, 5]], dim=1).view(-1, 3, 3)
             for R in rots:
                 m = R @ m @ R.T
             cov0 = torch.stack([m[:, 0, 0], m[:, 0, 1], m[:, 0, 2], m[:, 1, 1], m[:, 1, 2], m[:, 2, 2]], dim=1) * (scale_origin ** 2)
         gs_num = int(pos0.shape[0])
+        shs_render, opacity_render, n_render = init_shs, init_opacity, gs_num
         if sc.particle_filling is not None:
-            pos0, cov0 = self._fill(sc, pos0, cov0, n_grid, grid_lim)
+            pos0, cov0, filled_attrs = self._fill(sc, pos0, cov0, init_opacity, init_shs, n_grid, grid_lim)
+            if filled_attrs is not None:                     # visualize: every particle is a Gaussian from here on (:473-477)
+                shs_render, opacity_render = filled_attrs
+                n_render = int(pos0.shape[0])
+        n_filled = int(pos0.shape[0]) - gs_num
         vol = frame_export.get_particle_volume(pos0, n_grid, grid_lim / n_grid, unifrom=mp.get("material") == "sand")
         solver = MPM_Simulator_WARP(10, device=str(dev))
         solver.load_initial_data_from_torch(pos0, vol, cov0, n_grid=n_grid, grid_lim=grid_lim, device=str(dev))
@@ -191,14 +221,14 @@ class SceneBatchDriver:
         substep_dt = tp["substep_dt"]
         step_per_frame = int(tp["frame_dt"] / substep_dt)                                           # float division like :627
         frames_pos, frames_cov, frames_rgb = [], [], []
-        filled = gs_num != int(pos0.shape[0])
-        render = self._render_setup(sc, rots, scale_origin, original_mean_pos, gs_num) if sc.shs is not None and sc.camera_params is not None \
-            else None
+        filled = n_render != int(pos0.shape[0])
+        render = self._render_setup(sc, rots, scale_origin, original_mean_pos, shs_render, opacity_render, n_render, unselected) \
+            if sc.shs is not None and sc.camera_params is not None else None
         for frame in range(int(tp["frame_num"])):
             pos = solver.export_particle_x_to_torch()
             cov = solver.export_particle_cov_to_torch().view(-1, 6) if sc.cov is not None else None
             if filled:                                                                             # the Gaussians only (:591, 594)
-                pos, cov = pos[:gs_num], cov[:gs_num]
+                pos, cov = pos[:n_render], cov[:n_render]
             pr, cr = frame_export.render_frame_transform(pos, cov, sc.z_shift_value, scale_origin, original_mean_pos, rots)
             if render is not None:
                 image = render(frame, pr, cr)
@@ -214,23 +244,31 @@ class SceneBatchDriver:
             solver.p2g2p_n(step_per_frame, substep_dt)
         record = {"name": sc.name, "n_particles": int(pos0.shape[0]), "n_gaussians": gs_num, "frames_pos": frames_pos, "frames_cov": frames_cov,
                   "material_ids": props[4], "E": props[2], "substeps": step_per_frame * int(tp["frame_num"]), "time": solver.time,
-                  "bc_conditions": bc_conditions}
+                  "bc_conditions": bc_conditions, "n_filled": n_filled, "n_unselected": 0 if unselected is None else int(unselected["pos"].shape[0])}
         if render is not None:
             record["frames_rgb"] = frames_rgb
         return record
 
-    def _render_setup(self, sc: Scene, rots, scale_origin, original_mean_pos, gs_num: int):
+    def _render_setup(self, sc: Scene, rots, scale_origin, original_mean_pos, shs: torch.Tensor, opacity: torch.Tensor, n_render: int,
+                      unselected: Optional[Dict[str, torch.Tensor]]):
         """gs_simulation.py:529-540, 573-619: the view centre and orbit basis once, then per frame the camera for that frame
-        index and the Gaussians rasterised with their original opacity and SH (roll 0: the reference passes none)."""
+        index and the first n_render simulated particles rasterised with `shs` / `opacity` (the Gaussians' own, or with
+        `visualize` those of init_filled_particles), followed by the Gaussians outside sim_area, unchanged (roll 0: the
+        reference passes none)."""
         if sc.cov is None or sc.opacity is None:
             raise ValueError(f"scene {sc.name}: rendering needs the Gaussians' cov and opacity")
         if sc.cameras is None:
             raise ValueError(f"scene {sc.name}: rendering needs the model's cameras (the cameras.json list or its path)")
-        dev = self.device
-        shs = sc.shs.to(dev, torch.float32).contiguous()
-        opacity = sc.opacity.to(dev, torch.float32).reshape(-1).contiguous()
-        if shs.dim() != 3 or shs.shape[0] != gs_num or opacity.shape[0] != gs_num:
-            raise ValueError(f"scene {sc.name}: shs must be (N, K, 3) and opacity (N,) for the N = {gs_num} Gaussians")
+        shs = shs.contiguous()
+        opacity = opacity.reshape(-1).contiguous()
+        if shs.dim() != 3 or shs.shape[0] != n_render or opacity.shape[0] != n_render:
+            raise ValueError(f"scene {sc.name}: shs must be (N, K, 3) and opacity (N,) for the N = {n_render} Gaussians")
+        if unselected is not None:
+            u_shs, u_opacity = unselected["shs"], unselected["opacity"].reshape(-1)
+            if u_shs.dim() != 3 or u_shs.shape[1:] != shs.shape[1:]:
+                raise ValueError(f"scene {sc.name}: shs must be (N, K, 3)")
+            shs = torch.cat([shs, u_shs]).contiguous()
+            opacity = torch.cat([opacity, u_opacity]).contiguous()
         cp = gs_render.decode_camera_params(sc.camera_params)
         cams = gs_render.load_cameras(sc.cameras)
         center, basis = gs_render.get_center_view_worldspace_and_observant_coordinate(
@@ -240,26 +278,37 @@ class SceneBatchDriver:
         def render(frame: int, pos: torch.Tensor, cov: torch.Tensor) -> torch.Tensor:
             cam = gs_render.get_camera_view(cams, cp["default_camera_index"], center, basis, False, cp["init_azimuthm"], cp["init_elevation"],
                                             cp["init_radius"], None, cp["move_camera"], frame, cp["delta_a"], cp["delta_e"], cp["delta_r"])
+            if unselected is not None:                                                            # gs_simulation.py:602-606
+                pos, cov = torch.cat([pos, unselected["pos"]]), torch.cat([cov, unselected["cov"]])
             return gs_render.rasterize(pos, cov, opacity, cam, bg, shs=shs, sh_degree=sc.sh_degree)[0]
         return render
 
-    def _fill(self, sc: Scene, pos0: torch.Tensor, cov0: Optional[torch.Tensor], n_grid: int, grid_lim: float):
-        """Particle filling of gs_simulation.py:442-462, 479-480: the Gaussians first, then the filled particles with
-        covariance 0."""
+    def _fill(self, sc: Scene, pos0: torch.Tensor, cov0: Optional[torch.Tensor], opacity: Optional[torch.Tensor],
+              shs: Optional[torch.Tensor], n_grid: int, grid_lim: float):
+        """Particle filling of gs_simulation.py:442-462, 473-481: (positions, covariances, render attributes), the Gaussians
+        first, then the filled particles. Without `visualize` the filled particles get covariance 0 and the render
+        attributes are None; with it, each takes the SH, opacity and covariance of its nearest Gaussian
+        (init_filled_particles) and the render attributes are (shs, opacity) of all particles."""
         fp = particle_filling.decode_filling_params(sc.particle_filling, {"n_grid": n_grid})
-        if fp["smooth"] or fp["visualize"]:
+        if fp["smooth"]:
             raise NotImplementedError(
-                f"scene {sc.name}: particle filling with smooth / visualize needs mcubes.smooth (PyMCubes), which is not available")
-        if sc.opacity is None or cov0 is None:
+                f"scene {sc.name}: particle filling with smooth needs mcubes.smooth (PyMCubes), which is not available")
+        if opacity is None or cov0 is None:
             raise ValueError(f"scene {sc.name}: particle filling needs the Gaussians' opacity and cov")
+        if fp["visualize"] and shs is None:
+            raise ValueError(f"scene {sc.name}: particle filling with visualize needs the Gaussians' shs, opacity and cov")
         pos = particle_filling.fill_particles(
-            pos=pos0, opacity=sc.opacity.to(self.device, torch.float32), cov=cov0, grid_n=fp["n_grid"], max_samples=fp["max_particles_num"],
+            pos=pos0, opacity=opacity, cov=cov0, grid_n=fp["n_grid"], max_samples=fp["max_particles_num"],
             grid_dx=grid_lim / fp["n_grid"], density_thres=fp["density_threshold"], search_thres=fp["search_threshold"],
             max_particles_per_cell=fp["max_partciels_per_cell"], search_exclude_dir=fp["search_exclude_direction"],
             ray_cast_dir=fp["ray_cast_direction"], boundary=fp["boundary"], smooth=False)
+        n = pos0.shape[0]
+        if fp["visualize"]:
+            shs_all, opacity_all, cov = particle_filling.init_filled_particles(pos[:n], shs, cov0, opacity, pos[n:])
+            return pos, cov, (shs_all, opacity_all)
         cov = torch.zeros((pos.shape[0], 6), dtype=torch.float32, device=pos.device)
-        cov[:pos0.shape[0]] = cov0
-        return pos, cov
+        cov[:n] = cov0
+        return pos, cov, None
 
     # ------------------------------------------------------------------------------ batch
     def run(self, scenes: Sequence[Scene], out_dir: Optional[str] = None) -> List[Dict]:
