@@ -143,14 +143,24 @@ __global__ void mpm_select_box_kernel(const DevState s, float3 point, float3 siz
     const float ox = s.x[3 * p] - point.x, oy = s.x[3 * p + 1] - point.y, oz = s.x[3 * p + 2] - point.z;
     mask[p] = (fabsf(ox) < size.x && fabsf(oy) < size.y && fabsf(oz) < size.z) ? 1 : 0;
 }
+// Operands of the boundary-condition and selection comparisons. Each comparison flips a node's or a particle's whole value,
+// so they are computed in the reference's float32 operation order with one rounding per operation: nvcc would otherwise
+// contract them into FMAs, which round once and decide some nodes and particles differently (tests/test_mpm_bc_edges.py).
+// node coordinate minus a BC point: float(g) * dx - p
+__device__ __forceinline__ float bc_offset(int g, float dx, float p) { return __fsub_rn(__fmul_rn((float)g, dx), p); }
+// wp.dot: ((a.x b.x + a.y b.y) + a.z b.z)
+__device__ __forceinline__ float bc_dot(float ax, float ay, float az, float bx, float by, float bz) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(ax, bx), __fmul_rn(ay, by)), __fmul_rn(az, bz));
+}
+
 __global__ void mpm_select_cyl_kernel(const DevState s, float3 point, float3 normal, float half_height, float radius, int* mask) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= s.n) return;
     const float ox = s.x[3 * p] - point.x, oy = s.x[3 * p + 1] - point.y, oz = s.x[3 * p + 2] - point.z;
-    const float on = ox * normal.x + oy * normal.y + oz * normal.z;
+    const float on = bc_dot(ox, oy, oz, normal.x, normal.y, normal.z);
     const float vd = fabsf(on);
-    const float hx = ox - on * normal.x, hy = oy - on * normal.y, hz = oz - on * normal.z;
-    const float hd = sqrtf(hx * hx + hy * hy + hz * hz);
+    const float hx = __fsub_rn(ox, __fmul_rn(on, normal.x)), hy = __fsub_rn(oy, __fmul_rn(on, normal.y)), hz = __fsub_rn(oz, __fmul_rn(on, normal.z));
+    const float hd = sqrtf(bc_dot(hx, hy, hz, hx, hy, hz));
     mask[p] = (vd < half_height && hd < radius) ? 1 : 0;
 }
 

@@ -76,8 +76,13 @@ __device__ __forceinline__ void st_release_sys(int* p, int v) {
 
 struct AxisW { float w0, w1, w2, d0, d1, d2, fx; int b; };   // weights, derivative weights (without inv_dx), offset, base
 
-__device__ __forceinline__ AxisW axis_weights(float g) {
+// g = x * inv_dx is rounded once (__fmul_rn) before the base cell and fx use it, like the reference. Contracted into the
+// two subtractions, a product that rounds to exactly k + 0.5 gave base k - 1 with fx a hair under 1.5 (k a power of two):
+// node k - 1 then got a mass of ~1e-15 and a momentum from the weight gradient, and velocities up to 1e5
+// (tests/test_mpm_bc_edges.py, half-cell positions). Rounded first, the base is k and fx exactly 0.5, as in the reference.
+__device__ __forceinline__ AxisW axis_weights(float x, float inv_dx) {
     AxisW a;
+    const float g = __fmul_rn(x, inv_dx);
     a.b = (int)(g - 0.5f);                               // wp.int truncates toward zero (mpm_utils.py:344-346)
     const float fx = g - (float)a.b;
     a.fx = fx;
@@ -188,13 +193,15 @@ __device__ __forceinline__ void apply_modifier(const BC& bc, int orig, float tim
     if (bc.kind == PIXIE_BC_VELOCITY_TRANSLATION) {
         vx = bc.velocity[0]; vy = bc.velocity[1]; vz = bc.velocity[2];
     } else {                                                                             // rotation :1137-1179
+        // the half-plane test and the horizontal distance in the reference's operation order (bc_dot, no FMA)
         const float ox = px - bc.point[0], oy = py - bc.point[1], oz = pz - bc.point[2];
-        const float on = ox * bc.normal[0] + oy * bc.normal[1] + oz * bc.normal[2];
-        const float hx = ox - on * bc.normal[0], hy = oy - on * bc.normal[1], hz = oz - on * bc.normal[2];
-        const float hd = sqrtf(hx * hx + hy * hy + hz * hz);
-        const float cosine = (ox * bc.h1[0] + oy * bc.h1[1] + oz * bc.h1[2]) / hd;
+        const float on = bc_dot(ox, oy, oz, bc.normal[0], bc.normal[1], bc.normal[2]);
+        const float hx = __fsub_rn(ox, __fmul_rn(on, bc.normal[0])), hy = __fsub_rn(oy, __fmul_rn(on, bc.normal[1])),
+                    hz = __fsub_rn(oz, __fmul_rn(on, bc.normal[2]));
+        const float hd = sqrtf(bc_dot(hx, hy, hz, hx, hy, hz));
+        const float cosine = bc_dot(ox, oy, oz, bc.h1[0], bc.h1[1], bc.h1[2]) / hd;
         float theta = acosf(cosine);
-        if (!(ox * bc.h2[0] + oy * bc.h2[1] + oz * bc.h2[2] > 0.f)) theta = -theta;
+        if (!(bc_dot(ox, oy, oz, bc.h2[0], bc.h2[1], bc.h2[2]) > 0.f)) theta = -theta;
         const float a1 = -hd * sinf(theta) * bc.rotation_scale;
         const float a2 = hd * cosf(theta) * bc.rotation_scale;
         const float av = bc.translation_scale;
@@ -285,7 +292,7 @@ mpm_fused_kernel(const __grid_constant__ FusedState s, const float dt) {
         M3 F;
 #pragma unroll
         for (int k = 0; k < 9; ++k) F.m[k] = f[(FS_F + k) * cap + p];
-        const AxisW ax = axis_weights(px * s.inv_dx), ay = axis_weights(py * s.inv_dx), az = axis_weights(pz * s.inv_dx);
+        const AxisW ax = axis_weights(px, s.inv_dx), ay = axis_weights(py, s.inv_dx), az = axis_weights(pz, s.inv_dx);
         F3 v, Bx, By, Bz, Gx, Gy, Gz;
         const bool inside = ax.b >= 0 && ay.b >= 0 && az.b >= 0 && ax.b < n - 2 && ay.b < n - 2 && az.b < n - 2;   // (no b + 2: a blown-up
                                                                                                                   // position converts to INT_MAX)
@@ -382,7 +389,7 @@ mpm_fused_kernel(const __grid_constant__ FusedState s, const float dt) {
     }
 
     // ---------------------------------------------------------------------- p2g (mpm_utils.py:338-394), substep i+1
-    const AxisW ax = axis_weights(px * s.inv_dx), ay = axis_weights(py * s.inv_dx), az = axis_weights(pz * s.inv_dx);
+    const AxisW ax = axis_weights(px, s.inv_dx), ay = axis_weights(py, s.inv_dx), az = axis_weights(pz, s.inv_dx);
     const bool inside = ax.b >= 0 && ay.b >= 0 && az.b >= 0 && ax.b < n - 2 && ay.b < n - 2 && az.b < n - 2;   // (no b + 2: a blown-up
                                                                                                                   // position converts to INT_MAX)
     {   // RPIC damping of C (:374-379)
@@ -560,10 +567,10 @@ mpm_gridbox_kernel(const GridBoxArgs s, const float dt, const double dt_d) {
             const DevBC& bc = s.bcs[k];
             float q0 = s.pts_in[3 * k], q1 = s.pts_in[3 * k + 1], q2 = s.pts_in[3 * k + 2];
             if (bc.kind == PIXIE_BC_CUBOID && t >= (double)bc.start_time && t < (double)bc.end_time) {
-                // modify(): Python-float arithmetic, stored back as fp32 (mpm_solver_warp.py:899-905)
-                q0 = (float)((double)q0 + dt_d * (double)bc.velocity[0]);
-                q1 = (float)((double)q1 + dt_d * (double)bc.velocity[1]);
-                q2 = (float)((double)q2 + dt_d * (double)bc.velocity[2]);
+                // modify(): Python-float arithmetic (unfused), stored back as fp32 (mpm_solver_warp.py:899-905)
+                q0 = (float)__dadd_rn((double)q0, __dmul_rn(dt_d, (double)bc.velocity[0]));
+                q1 = (float)__dadd_rn((double)q1, __dmul_rn(dt_d, (double)bc.velocity[1]));
+                q2 = (float)__dadd_rn((double)q2, __dmul_rn(dt_d, (double)bc.velocity[2]));
             }
             s.pts_out[3 * k] = q0; s.pts_out[3 * k + 1] = q1; s.pts_out[3 * k + 2] = q2;
         }
@@ -595,14 +602,16 @@ mpm_gridbox_kernel(const GridBoxArgs s, const float dt, const double dt_d) {
         if (s.grid_v_damping_scale < 1.0f) {                   // add_damping_via_grid :583-588 (only if < 1)
             vx *= s.grid_v_damping_scale; vy *= s.grid_v_damping_scale; vz *= s.grid_v_damping_scale;
         }
+        // every BC decision below is a float32 comparison that flips the node's whole value, so its operands are computed
+        // like the reference's: one rounding per operation, no FMA contraction (bc_offset / bc_dot)
         for (int k = 0; k < s.n_bc; ++k) {
             const DevBC& bc = s.bcs[k];
             if (bc.kind > PIXIE_BC_BOUNDING_BOX) continue;
             const bool active = time >= bc.start_time && time < bc.end_time;
             if (bc.kind == PIXIE_BC_SURFACE_COLLIDER) {        // :785-840
                 if (active) {
-                    const float ox = (float)gx * s.dx - s.pts_in[3 * k], oy = (float)gy * s.dx - s.pts_in[3 * k + 1], oz = (float)gz * s.dx - s.pts_in[3 * k + 2];
-                    if (ox * bc.normal[0] + oy * bc.normal[1] + oz * bc.normal[2] < 0.0f) {
+                    const float ox = bc_offset(gx, s.dx, s.pts_in[3 * k]), oy = bc_offset(gy, s.dx, s.pts_in[3 * k + 1]), oz = bc_offset(gz, s.dx, s.pts_in[3 * k + 2]);
+                    if (bc_dot(ox, oy, oz, bc.normal[0], bc.normal[1], bc.normal[2]) < 0.0f) {
                         if (bc.surface_type == 11) {
                             const float zz = (float)gz * s.dx;
                             if (zz < 0.4f || zz > 0.53f) { vx = 0.f; vy = 0.f; vz = 0.f; }
@@ -616,12 +625,12 @@ mpm_gridbox_kernel(const GridBoxArgs s, const float dt, const double dt_d) {
                 }
             } else if (bc.kind == PIXIE_BC_CUBOID) {           // :874-897
                 if (active) {
-                    const float ox = (float)gx * s.dx - s.pts_in[3 * k], oy = (float)gy * s.dx - s.pts_in[3 * k + 1], oz = (float)gz * s.dx - s.pts_in[3 * k + 2];
+                    const float ox = bc_offset(gx, s.dx, s.pts_in[3 * k]), oy = bc_offset(gy, s.dx, s.pts_in[3 * k + 1]), oz = bc_offset(gz, s.dx, s.pts_in[3 * k + 2]);
                     if (fabsf(ox) < bc.size[0] && fabsf(oy) < bc.size[1] && fabsf(oz) < bc.size[2]) {
                         vx = bc.velocity[0]; vy = bc.velocity[1]; vz = bc.velocity[2];
                     }
                 } else if (bc.reset == 1) {
-                    if (time < bc.end_time + 15.0f * dt) { vx = 0.f; vy = 0.f; vz = 0.f; }
+                    if (time < __fadd_rn(bc.end_time, __fmul_rn(15.0f, dt))) { vx = 0.f; vy = 0.f; vz = 0.f; }
                 }
             } else {                                           // bounding box :917-974
                 if (active) {
@@ -647,8 +656,8 @@ __global__ void fs_key_kernel(const float* __restrict__ x, long long stride_comp
                               int* __restrict__ keys, int* __restrict__ idx) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= n) return;
-    const AxisW ax = axis_weights(x[0 * stride_comp + p * stride_part] * inv_dx), ay = axis_weights(x[1 * stride_comp + p * stride_part] * inv_dx),
-                az = axis_weights(x[2 * stride_comp + p * stride_part] * inv_dx);
+    const AxisW ax = axis_weights(x[0 * stride_comp + p * stride_part], inv_dx), ay = axis_weights(x[1 * stride_comp + p * stride_part], inv_dx),
+                az = axis_weights(x[2 * stride_comp + p * stride_part], inv_dx);
     const int bx = min(max(ax.b, 0), n_grid - 1), by = min(max(ay.b, 0), n_grid - 1), bz = min(max(az.b, 0), n_grid - 1);
     keys[p] = (bx * n_grid + by) * n_grid + bz;
     idx[p] = p;
@@ -670,7 +679,7 @@ __global__ void fs_box_kernel(const float* __restrict__ x, long long stride_comp
     for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
 #pragma unroll
         for (int a = 0; a < 3; ++a) {
-            const AxisW w = axis_weights(x[a * stride_comp + p * stride_part] * inv_dx);
+            const AxisW w = axis_weights(x[a * stride_comp + p * stride_part], inv_dx);
             lo[a] = min(lo[a], max(w.b, 0));
             hi[a] = max(hi[a], min(max(w.b, 0), n_grid - 3) + 3);
         }
@@ -690,7 +699,7 @@ __global__ void fs_excursion_kernel(const float* __restrict__ x, long long strid
                                     int* __restrict__ out) {
     int e = 0;
     for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
-        const int b = axis_weights(x[p * stride_part] * inv_dx).b;
+        const int b = axis_weights(x[p * stride_part], inv_dx).b;
         e = max(e, max(lo - b, b - (hi - 1)));
     }
     for (int o = 16; o > 0; o >>= 1) e = max(e, __shfl_xor_sync(0xffffffffu, e, o));

@@ -32,6 +32,71 @@ NAME_TO_MATERIAL_ID.update({"elastic": 0, "rigid": 6})
 MAX_BCS = 256
 
 
+# ---- host-side BC parameter arithmetic of the reference (:749-1210). The reference evaluates it at Python scope, where
+# `wp.sqrt` / `wp.abs` / `wp.length` return float32 scalars and wp.vec3 arithmetic is float32 with one rounding per
+# operation; a Python float combined with a float32 scalar is rounded to float32 first. The BC kernels then compare node
+# and particle coordinates against these values, so they are reproduced bit for bit (tests/test_mpm_bc_edges.py).
+_f32 = np.float32
+
+
+def _dot_f32(a, b):
+    """wp.dot of two float32 3-vectors: ((a0 b0 + a1 b1) + a2 b2), one rounding per operation."""
+    acc = _f32(0.0)
+    for k in range(3):
+        acc = _f32(acc + _f32(_f32(a[k]) * _f32(b[k])))
+    return acc
+
+
+def _unit_normal_f32(normal):
+    """`normal_scale = 1.0 / wp.sqrt(float(...))`, then `normal_scale * x` per component (:760-761, :1092-1095)."""
+    scale = _f32(_f32(1.0) / _f32(np.sqrt(_f32(float(normal[0] ** 2 + normal[1] ** 2 + normal[2] ** 2)))))
+    return np.array([_f32(scale * _f32(x)) for x in normal], dtype=_f32)
+
+
+def collider_normal(normal) -> np.ndarray:
+    """The float32 normal `add_surface_collider` stores (:758-768)."""
+    return _unit_normal_f32(normal)
+
+
+def rotation_axes(normal):
+    """(normal, horizontal_axis_1, horizontal_axis_2) as `enforce_particle_velocity_rotation` stores them (:1092-1117)."""
+    n = _unit_normal_f32(normal)
+    h1 = np.array([1.0, 1.0, 1.0], dtype=_f32)
+    if _f32(np.abs(_dot_f32(n, h1))) < _f32(0.01):
+        h1 = np.array([0.72, 0.37, -0.67], dtype=_f32)
+    d = _dot_f32(h1, n)
+    h1 = np.array([_f32(h1[k] - _f32(d * n[k])) for k in range(3)], dtype=_f32)
+    inv = _f32(_f32(1.0) / _f32(np.sqrt(_dot_f32(h1, h1))))
+    h1 = np.array([_f32(h1[k] * inv) for k in range(3)], dtype=_f32)
+    h2 = np.cross(h1, n).astype(_f32)              # float32 a_i b_j - a_j b_i, like wp.cross
+    return n, h1, h2
+
+
+def release_layers(normal, start_position, end_position, end_time, num_layers=50):
+    """(point, size, end_time) of the translation modifiers `release_particles_sequentially` registers (:1185-1210):
+    the layer half-length is float32 (`wp.abs(...) / num_layers`), the end times are Python floats."""
+    point, size, axis = [0, 0, 0], [0, 0, 0], -1
+    for i in range(3):
+        if normal[i] == 0:
+            point[i] = 1
+            size[i] = 1
+        else:
+            axis = i
+            point[i] = end_position
+    half_length_portion = _f32(_f32(np.abs(_f32(start_position - end_position))) / _f32(num_layers))
+    end_time_portion = end_time / num_layers
+    out = []
+    for i in range(num_layers):
+        size[axis] = _f32(half_length_portion * _f32(num_layers - i))
+        out.append((list(point), list(size), end_time_portion * (i + 1)))
+    return out
+
+
+def impulse_end_time(start_time, dt, num_dt):
+    """`start_time + dt * num_dt` in Python floats, stored as float32 (:993-994)."""
+    return start_time + dt * num_dt
+
+
 def get_material_name(material_id):
     """Reference quirk kept: despite its name this maps a material NAME to its id (:29-39)."""
     return NAME_TO_MATERIAL_ID.get(material_id, -1)
@@ -438,8 +503,7 @@ class MPM_Simulator_WARP:
     def add_surface_collider(self, point, normal, surface="sticky", friction=0.0, start_time=0.0, end_time=999.0):
         """:749-843."""
         point = list(point)
-        normal_scale = 1.0 / math.sqrt(float(sum(x ** 2 for x in normal)))
-        normal = list(normal_scale * x for x in normal)
+        normal = collider_normal(normal)
         if surface == "sticky" and friction != 0:
             raise ValueError("friction must be 0 on sticky surfaces.")
         surface_type = {"sticky": 0, "slip": 1, "cut": 11}.get(surface, 2)
@@ -469,7 +533,7 @@ class MPM_Simulator_WARP:
         """:982-1029."""
         mask = self._select_box(point, size)
         bc = self._add_bc(_lib.BC_IMPULSE, mask=mask, point=point, size=size, velocity=force, start_time=start_time,
-                          end_time=start_time + dt * num_dt)
+                          end_time=impulse_end_time(start_time, dt, num_dt))
         self.impulse_params.append(bc)
         self.pre_p2g_operations.append("apply_force")
 
@@ -484,15 +548,7 @@ class MPM_Simulator_WARP:
     def enforce_particle_velocity_rotation(self, point, normal, half_height_and_radius, rotation_scale,
                                            translation_scale, start_time, end_time, device="cuda:0"):
         """:1080-1179 (axes built in fp32 like the wp.vec3 arithmetic of the reference)."""
-        f32 = np.float32
-        normal_scale = 1.0 / math.sqrt(float(normal[0] ** 2 + normal[1] ** 2 + normal[2] ** 2))
-        n = np.asarray([normal_scale * x for x in normal], dtype=f32)
-        h1 = np.asarray([1.0, 1.0, 1.0], dtype=f32)
-        if abs(float(np.dot(n, h1))) < 0.01:
-            h1 = np.asarray([0.72, 0.37, -0.67], dtype=f32)
-        h1 = (h1 - np.dot(h1, n) * n).astype(f32)
-        h1 = (h1 * f32(1.0 / np.linalg.norm(h1))).astype(f32)
-        h2 = np.cross(h1, n).astype(f32)
+        n, h1, h2 = rotation_axes(normal)
         mask = torch.zeros(self.n_particles, dtype=torch.int32, device=self._device)
         p3, n3 = (C.c_float * 3)(*[float(v) for v in point]), (C.c_float * 3)(*[float(v) for v in n])
         _lib.check(_lib.load().pixie_mpm_select_cylinder(self._handle, p3, n3, float(half_height_and_radius[0]),
@@ -507,18 +563,6 @@ class MPM_Simulator_WARP:
 
     def release_particles_sequentially(self, normal, start_position, end_position, num_layers, start_time, end_time):
         """:1183-1210 (num_layers is overridden to 50, as in the reference)."""
-        num_layers = 50
-        point, size, axis = [0, 0, 0], [0, 0, 0], -1
-        for i in range(3):
-            if normal[i] == 0:
-                point[i] = 1
-                size[i] = 1
-            else:
-                axis = i
-                point[i] = end_position
-        half_length_portion = abs(start_position - end_position) / num_layers
-        end_time_portion = end_time / num_layers
-        for i in range(num_layers):
-            size[axis] = half_length_portion * (num_layers - i)
+        for point, size, layer_end in release_layers(normal, start_position, end_position, end_time):
             self.enforce_particle_velocity_translation(point=point, size=size, velocity=[0, 0, 0],
-                                                       start_time=start_time, end_time=end_time_portion * (i + 1))
+                                                       start_time=start_time, end_time=layer_end)
