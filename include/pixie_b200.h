@@ -125,6 +125,16 @@ int pixie_particle_volume(const float* pos_dev, int n, int grid_n, float grid_dx
 int pixie_frame_transform(const float* pos_dev, const float* cov_dev, int n, float z_shift_value, float scale_origin,
                           const float original_mean_pos_host[3], const float* rotations_host, int n_rot, float* pos_out_dev,
                           float* cov_out_dev, void* stream);
+/* pixie_gaussian_ply_records: one 3DGS PLY vertex per Gaussian, as export_gaussians_to_ply (gs_simulation.py:290-322) with
+ * cov3D_to_log_scales_and_quats (:253-288) and GaussianModel.save_ply / construct_list_of_attributes
+ * (gaussian-splatting/scene/gaussian_model.py:177-208) write it. records_dev [n][14 + 3K] fp32: x y z, nx ny nz (0),
+ * f_dc_0..2 = shs[p][0][0..2], f_rest_{c (K-1) + k - 1} = shs[p][k][c] (k >= 1), opacity, scale_0..2, rot_0..3. The scales
+ * are log sqrt(max(lambda, 1e-12)) of the covariance's eigenvalues in descending order; rot is the quaternion (w, x, y, z)
+ * of R = the eigenvectors as columns, the third negated when det R < 0, by scipy's Rotation.from_matrix (Markley's
+ * decision, so w may be negative). pos_dev [n][3], cov_dev [n][6] upper triangle (xx xy xz yy yz zz), shs_dev [n][K][3]
+ * with K in {1, 4, 9, 16}, opacity_dev [n]. Stream-ordered, no host sync. */
+int pixie_gaussian_ply_records(const float* pos_dev, const float* cov_dev, const float* shs_dev, int K, const float* opacity_dev, int n,
+                               float* records_dev, void* stream);
 /* ---- particle filling of hollow Gaussian objects (PG/particle_filling/filling.py:26-380, Taichi in the reference).
  * pixie_fill_density: densify_grids (:26-87). count_dev [grid_n^3] int32 = Gaussians per cell (a Gaussian outside the grid
  * counts in the nearest border cell; the reference indexes out of range), density_dev [grid_n^3] fp32 = sum over the

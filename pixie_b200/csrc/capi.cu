@@ -8,6 +8,7 @@
 #include "particle_fill.cuh"
 #include "nearest.cuh"
 #include "gs_render.cuh"
+#include "gs_ply.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -139,6 +140,15 @@ int pixie_frame_transform(const float* pos, const float* cov, int n, float z_shi
     if (n_rot < 0 || n_rot > 8) return set_err("frame_transform: at most 8 rotations");
     if (require_device()) return 1;
     if (pixie::frame_transform(pos, cov, n, z_shift, scale, mean, rotations, n_rot, pos_out, cov_out, (cudaStream_t)stream)) return set_err("frame_transform failed");
+    return 0;
+}
+int pixie_gaussian_ply_records(const float* pos, const float* cov, const float* shs, int K, const float* opacity, int n, float* records,
+                               void* stream) {
+    if (n < 0) return set_err("gaussian_ply_records: negative point count");
+    if (K != 1 && K != 4 && K != 9 && K != 16) return set_err("gaussian_ply_records: K must be 1, 4, 9 or 16 SH coefficients");
+    if (n > 0 && (!pos || !cov || !shs || !opacity || !records)) return set_err("null argument");
+    if (require_device()) return 1;
+    if (pixie::gaussian_ply_records(pos, cov, shs, K, opacity, n, records, (cudaStream_t)stream)) return set_err("gaussian_ply_records failed");
     return 0;
 }
 // n^3 cells and their offsets are int32 on the device

@@ -14,6 +14,7 @@ per scene, none of it arithmetic. Here the two networks and one solver stay resi
     kNN smoothing (+ ground / stationary cuboids) + upload (apply_material_field_to_simulation) [material_field.py:295-550]
     frame loop: export positions / covariances in the Gaussians' frame, step_per_frame x p2g2p [gs_simulation.py:585-634]
     + the rendered frame, when the scene has SH coefficients and camera parameters         [gs_simulation.py:573-619]
+    + the frame's Gaussians as a 3DGS PLY, when the scene sets save_ply                    [gs_simulation.py:621-628]
 
 Function names and argument meaning follow those reference functions; image / video files, Hydra and the file layout stay
 outside.
@@ -22,6 +23,7 @@ data-path collective.
 """
 from __future__ import annotations
 
+import contextlib
 import os
 from dataclasses import dataclass, field
 from typing import Callable, Dict, Iterable, List, Optional, Sequence
@@ -70,6 +72,11 @@ class Scene:
     camera_params: Optional[Dict] = None           # the config's camera keys, raw or decode_camera_params'd
     cameras: object = None                         # the model's cameras.json list, or its path
     white_bg: bool = False
+    # --save_ply (gs_simulation.py:621-628): every frame's rendered Gaussians as <ply_dir>/frame_{frame:05d}.ply; needs
+    # shs, opacity and cov, not the cameras. to_original_coord (decode_param.py:128-131 default) writes the Gaussians'
+    # frame positions; off, the solver's positions (the covariances stay in the Gaussians' frame either way)
+    save_ply: bool = False
+    to_original_coord: bool = True
 
 
 def transform2origin(position_tensor: torch.Tensor):
@@ -151,13 +158,21 @@ class SceneBatchDriver:
     # ------------------------------------------------------------------------------ physics half
     def run_physics_simulation(self, sc: Scene, cloud: Dict[str, torch.Tensor],
                                on_frame: Optional[Callable[[int, torch.Tensor, Optional[torch.Tensor]], None]] = None,
-                               on_image: Optional[Callable[[int, torch.Tensor], None]] = None) -> Dict:
+                               on_image: Optional[Callable[[int, torch.Tensor], None]] = None, ply_dir: Optional[str] = None) -> Dict:
         """One scene's rollout (gs_simulation.py:395-634): returns the per-frame render-space positions (and covariances when
         the scene has them) unless `on_frame(frame, pos, cov)` consumes them. A scene with `shs` and `camera_params` is also
         rendered each frame (the Gaussians only, from the frame's camera); the (3, H, W) images go to `on_image(frame, image)`
         or to the record's `frames_rgb`. With `sim_area`, only the Gaussians inside it are simulated and exported; the others
         are appended, unchanged, to every rendered frame. With the filling block's `visualize`, the filled particles carry
-        their nearest Gaussian's SH, opacity and covariance and are exported and rendered like Gaussians."""
+        their nearest Gaussian's SH, opacity and covariance and are exported and rendered like Gaussians. With `save_ply`,
+        each frame's rendered particles (not the Gaussians outside sim_area) with their render SH and opacity are also
+        written to `ply_dir/frame_{frame:05d}.ply` (export_gaussians_to_ply's file), the copy and the write overlapping the
+        next frame's substeps; existing files there are overwritten, nothing is deleted."""
+        if sc.save_ply:
+            if sc.shs is None or sc.opacity is None or sc.cov is None:
+                raise ValueError(f"scene {sc.name}: save_ply needs the Gaussians' shs, opacity and cov")
+            if ply_dir is None:
+                raise ValueError(f"scene {sc.name}: save_ply needs a ply_dir")
         dev = self.device
         mp, tp = dict(sc.material_params), sc.time_params
         n_grid, grid_lim = int(mp.get("n_grid", 64)), float(mp.get("grid_lim", 2.0))
@@ -224,24 +239,27 @@ class SceneBatchDriver:
         filled = n_render != int(pos0.shape[0])
         render = self._render_setup(sc, rots, scale_origin, original_mean_pos, shs_render, opacity_render, n_render, unselected) \
             if sc.shs is not None and sc.camera_params is not None else None
-        for frame in range(int(tp["frame_num"])):
-            pos = solver.export_particle_x_to_torch()
-            cov = solver.export_particle_cov_to_torch().view(-1, 6) if sc.cov is not None else None
-            if filled:                                                                             # the Gaussians only (:591, 594)
-                pos, cov = pos[:n_render], cov[:n_render]
-            pr, cr = frame_export.render_frame_transform(pos, cov, sc.z_shift_value, scale_origin, original_mean_pos, rots)
-            if render is not None:
-                image = render(frame, pr, cr)
-                if on_image is not None:
-                    on_image(frame, image)
+        with frame_export.PlyFrameWriter(ply_dir, dev) if sc.save_ply else contextlib.nullcontext() as ply:
+            for frame in range(int(tp["frame_num"])):
+                pos = solver.export_particle_x_to_torch()
+                cov = solver.export_particle_cov_to_torch().view(-1, 6) if sc.cov is not None else None
+                if filled:                                                                         # the Gaussians only (:591, 594)
+                    pos, cov = pos[:n_render], cov[:n_render]
+                pr, cr = frame_export.render_frame_transform(pos, cov, sc.z_shift_value, scale_origin, original_mean_pos, rots)
+                if render is not None:
+                    image = render(frame, pr, cr)
+                    if on_image is not None:
+                        on_image(frame, image)
+                    else:
+                        frames_rgb.append(image)
+                if ply is not None:                                                                # export_gaussians_to_ply
+                    ply.submit(frame, pr if sc.to_original_coord else pos, cr, shs_render, opacity_render)
+                if on_frame is not None:
+                    on_frame(frame, pr, cr)
                 else:
-                    frames_rgb.append(image)
-            if on_frame is not None:
-                on_frame(frame, pr, cr)
-            else:
-                frames_pos.append(pr.clone())
-                frames_cov.append(None if cr is None else cr.clone())
-            solver.p2g2p_n(step_per_frame, substep_dt)
+                    frames_pos.append(pr.clone())
+                    frames_cov.append(None if cr is None else cr.clone())
+                solver.p2g2p_n(step_per_frame, substep_dt)
         record = {"name": sc.name, "n_particles": int(pos0.shape[0]), "n_gaussians": gs_num, "frames_pos": frames_pos, "frames_cov": frames_cov,
                   "material_ids": props[4], "E": props[2], "substeps": step_per_frame * int(tp["frame_num"]), "time": solver.time,
                   "bc_conditions": bc_conditions, "n_filled": n_filled, "n_unselected": 0 if unselected is None else int(unselected["pos"].shape[0])}
@@ -312,8 +330,10 @@ class SceneBatchDriver:
 
     # ------------------------------------------------------------------------------ batch
     def run(self, scenes: Sequence[Scene], out_dir: Optional[str] = None) -> List[Dict]:
-        """This rank's share of `scenes` end to end; returns one record per processed scene (in scene order)."""
+        """This rank's share of `scenes` end to end; returns one record per processed scene (in scene order). A scene with
+        save_ply writes its frames to `<out_dir>/<scene>/ply_files`."""
         rank, world, _ = dist_utils.env_rank_world()
         mine = [scenes[i] for i in dict.fromkeys(dist_utils.shard_scenes(len(scenes), rank, world))]
         clouds = self.generate_neural_segmentation(mine, out_dir)
-        return [self.run_physics_simulation(sc, cl) for sc, cl in zip(mine, clouds)]
+        return [self.run_physics_simulation(sc, cl, ply_dir=None if out_dir is None else os.path.join(out_dir, sc.name, "ply_files"))
+                for sc, cl in zip(mine, clouds)]
