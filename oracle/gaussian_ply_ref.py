@@ -18,16 +18,27 @@ _FULL_FROM_UPPER = [0, 1, 2, 1, 3, 4, 2, 4, 5]
 
 
 def cov3D_to_log_scales_and_quats(cov3D):
-    """(log_scales (N, 3), quats_wxyz (N, 4)) in float64 from (N, 6) upper-triangular covariances."""
+    """(log_scales (N, 3), quats_wxyz (N, 4)) in float64 from (N, 6) upper-triangular covariances. A row with a NaN or
+    +-Inf entry gives NaN log scales and quaternion (the product's convention; the reference raises or returns NaN)."""
+    u = np.asarray(cov3D, np.float64).reshape(-1, 6)
+    bad = ~np.isfinite(u).all(axis=1)
+    evals, R = eigen_frame(np.where(bad[:, None], 0.0, u))
+    ls, q = np.log(np.sqrt(np.maximum(evals, 1e-12))), quat_wxyz_from_matrix(R)
+    ls[bad], q[bad] = np.nan, np.nan
+    return ls, q
+
+
+def eigen_frame(cov3D):
+    """(eigenvalues (N, 3) descending, R (N, 3, 3)) of finite (N, 6) covariances in fp64: the eigenvectors as columns,
+    the third negated where det R < 0, as cov3D_to_log_scales_and_quats hands R to from_matrix."""
     m = np.asarray(cov3D, np.float64).reshape(-1, 6)[:, _FULL_FROM_UPPER].reshape(-1, 3, 3)
     evals, evecs = np.linalg.eigh(m)                                       # ascending
     idx = np.argsort(-evals, axis=1, kind="stable")
     evals = np.take_along_axis(evals, idx, axis=1)
     R = np.take_along_axis(evecs, idx[:, None, :], axis=2).copy()
-    log_scales = np.log(np.sqrt(np.maximum(evals, 1e-12)))
     neg = np.linalg.det(R) < 0
     R[neg, :, 2] *= -1
-    return log_scales, quat_wxyz_from_matrix(R)
+    return evals, R
 
 
 def quat_wxyz_from_matrix(R):

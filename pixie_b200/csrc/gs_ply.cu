@@ -15,7 +15,7 @@ namespace pixie {
 namespace {
 
 constexpr int kThreads = 128;
-constexpr int kMaxSweeps = 10;        // a 3x3 converges in 4-6 cyclic sweeps; the cap bounds NaN / Inf inputs
+constexpr int kMaxSweeps = 10;        // a 3x3 converges in 4-6 cyclic sweeps; the cap bounds the loop
 
 // A <- J^T A J, V <- V J for the rotation J that zeroes A[P][Q] (Numerical Recipes' `jacobi` step); R is the third index
 template <int P, int Q, int R>
@@ -48,14 +48,23 @@ __device__ __forceinline__ void swap_pair(double (&lam)[3], double (&V)[3][3], i
 }
 
 // cov3D_to_log_scales_and_quats for one upper-triangular covariance u = (xx, xy, xz, yy, yz, zz):
-// out = (log s0, log s1, log s2, w, x, y, z)
+// out = (log s0, log s1, log s2, w, x, y, z); all seven NaN when any entry of u is NaN or +-Inf (the Jacobi below would
+// stop on a NaN at once and fmax would turn a NaN eigenvalue into the clamp, writing a plausible Gaussian instead)
 __device__ __forceinline__ void cov_to_scales_quat(const float* u, float* out) {
+    bool finite = true;
+#pragma unroll
+    for (int i = 0; i < 6; ++i) finite &= isfinite(u[i]);
+    if (!finite) {
+#pragma unroll
+        for (int i = 0; i < 7; ++i) out[i] = __int_as_float(0x7fc00000);
+        return;
+    }
     double A[3][3] = {{u[0], u[1], u[2]}, {u[1], u[3], u[4]}, {u[2], u[4], u[5]}};
     double V[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
     for (int sweep = 0; sweep < kMaxSweeps; ++sweep) {
         const double off = A[0][1] * A[0][1] + A[0][2] * A[0][2] + A[1][2] * A[1][2];
         const double diag = A[0][0] * A[0][0] + A[1][1] * A[1][1] + A[2][2] * A[2][2];
-        if (!(off > 1e-36 * diag)) break;                   // also ends a zero matrix and NaN input
+        if (!(off > 1e-36 * diag)) break;                   // also ends a zero matrix
         jacobi_rotate<0, 1, 2>(A, V);
         jacobi_rotate<0, 2, 1>(A, V);
         jacobi_rotate<1, 2, 0>(A, V);

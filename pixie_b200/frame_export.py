@@ -91,7 +91,8 @@ def gaussian_ply_records(pos: torch.Tensor, cov: torch.Tensor, shs: torch.Tensor
     """The (N, 14 + 3K) float32 PLY vertex rows of N Gaussians, on their device: pos (N, 3), cov (N, 6) upper triangle,
     shs (N, K, 3) with K in {1, 4, 9, 16}, opacity N values. Columns in gaussian_ply_attributes(K) order: pos, zero
     normals, shs[:, 0], shs[:, 1:] transposed to (3, K - 1) and flattened, opacity, the log scales and the (w, x, y, z)
-    quaternion of cov3D_to_log_scales_and_quats. One kernel, stream-ordered on the current stream."""
+    quaternion of cov3D_to_log_scales_and_quats. A covariance with a NaN or +-Inf entry gives NaN log scales and a NaN
+    quaternion in its row; its other columns are copied as they are. One kernel, stream-ordered on the current stream."""
     lib = _lib.require_device()
     if not pos.is_cuda:
         raise _lib.PixieError("gaussian_ply_records requires CUDA tensors; there is no CPU fallback")
@@ -131,7 +132,7 @@ def cov3D_to_log_scales_and_quats(cov3D: torch.Tensor) -> Tuple[torch.Tensor, to
 def _write_ply(path: str, header: bytes, rows) -> None:
     with open(path, "wb") as f:
         f.write(header)
-        f.write(memoryview(rows.numpy()).cast("B"))
+        f.write(rows.numpy())                    # raw bytes, no copy; an empty frame writes the header alone
 
 
 def export_gaussians_to_ply(ply_out_dir, mpm_solver, active_sh_degree, gs_num, scale_origin, rotation_matrices, opacity_render,
