@@ -135,6 +135,19 @@ int pixie_frame_transform(const float* pos_dev, const float* cov_dev, int n, flo
  * with K in {1, 4, 9, 16}, opacity_dev [n]. Stream-ordered, no host sync. */
 int pixie_gaussian_ply_records(const float* pos_dev, const float* cov_dev, const float* shs_dev, int K, const float* opacity_dev, int n,
                                float* records_dev, void* stream);
+/* pixie_gaussian_checkpoint_decode: a trained 3DGS checkpoint, as GaussianModel.load_ply
+ * (gaussian-splatting/scene/gaussian_model.py:215-260) then get_xyz, get_features, get_opacity and get_covariance() give it,
+ * optionally filtered by gs_simulation.py:405. table_dev: the PLY's binary little-endian vertex element as it is in the file,
+ * n rows of row_bytes bytes (a multiple of 4). cols [11 + 3K] host: the byte offsets within a row of the float32 columns
+ * x y z, f_dc_0..2, f_rest_0..3(K-1)-1 (in numeric order), opacity, scale_0..2, rot_0..3; each a multiple of 4. K in
+ * {1, 4, 9, 16}. Outputs, capacity n rows each: pos_dev [.][3], shs_dev [.][K][3] (shs[p][0][c] = f_dc_c,
+ * shs[p][k][c] = f_rest_{c (K-1) + k - 1}), opacity_dev [.] = sigmoid(opacity), cov_dev [.][6] = the upper triangle
+ * (xx xy xz yy yz zz) of L L^T, L = build_rotation(rot) diag(exp(scale)). With has_threshold only the rows with
+ * opacity > threshold (float32, strict, NaN dropped) are written, compacted in file order; *m_host receives their number
+ * (n without a threshold). Host-synchronises on the stream once when filtering. */
+int pixie_gaussian_checkpoint_decode(const void* table_dev, long long n, int row_bytes, const int* cols, int K, int has_threshold,
+                                     float threshold, float* pos_dev, float* shs_dev, float* opacity_dev, float* cov_dev,
+                                     long long* m_host, void* stream);
 /* ---- particle filling of hollow Gaussian objects (PG/particle_filling/filling.py:26-380, Taichi in the reference).
  * pixie_fill_density: densify_grids (:26-87). count_dev [grid_n^3] int32 = Gaussians per cell (a Gaussian outside the grid
  * counts in the nearest border cell; the reference indexes out of range), density_dev [grid_n^3] fp32 = sum over the

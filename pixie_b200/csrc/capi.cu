@@ -9,6 +9,7 @@
 #include "nearest.cuh"
 #include "gs_render.cuh"
 #include "gs_ply.cuh"
+#include "gs_load.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -149,6 +150,34 @@ int pixie_gaussian_ply_records(const float* pos, const float* cov, const float* 
     if (n > 0 && (!pos || !cov || !shs || !opacity || !records)) return set_err("null argument");
     if (require_device()) return 1;
     if (pixie::gaussian_ply_records(pos, cov, shs, K, opacity, n, records, (cudaStream_t)stream)) return set_err("gaussian_ply_records failed");
+    return 0;
+}
+int pixie_gaussian_checkpoint_decode(const void* table, long long n, int row_bytes, const int* cols, int K, int has_threshold, float threshold,
+                                     float* pos, float* shs, float* opacity, float* cov, long long* m_host, void* stream) {
+    if (!cols || !m_host || (n > 0 && (!table || !pos || !shs || !opacity || !cov))) return set_err("null argument");
+    if (n < 0) return set_err("gaussian_checkpoint_decode: negative row count");
+    if (K != 1 && K != 4 && K != 9 && K != 16) return set_err("gaussian_checkpoint_decode: K must be 1, 4, 9 or 16 SH coefficients");
+    if (row_bytes < 4 || row_bytes % 4 != 0 || row_bytes / 4 > pixie::kGsLoadMaxRowWords)
+        return set_err("gaussian_checkpoint_decode: the row stride must be a multiple of 4 bytes, at most " +
+                       std::to_string(4 * pixie::kGsLoadMaxRowWords));
+    const int row_words = row_bytes / 4, n_cols = 11 + 3 * K;
+    pixie::GsColumns c{};
+    int* dst[59];
+    int k = 0;
+    for (int i = 0; i < 3; ++i) dst[k++] = &c.xyz[i];
+    for (int i = 0; i < 3; ++i) dst[k++] = &c.dc[i];
+    for (int i = 0; i < 3 * (K - 1); ++i) dst[k++] = &c.rest[i];
+    dst[k++] = &c.opacity;
+    for (int i = 0; i < 3; ++i) dst[k++] = &c.scale[i];
+    for (int i = 0; i < 4; ++i) dst[k++] = &c.rot[i];
+    for (int i = 0; i < n_cols; ++i) {
+        if (cols[i] < 0 || cols[i] % 4 != 0 || cols[i] / 4 >= row_words)
+            return set_err("gaussian_checkpoint_decode: column " + std::to_string(i) + " is not a 4-byte aligned offset inside the row");
+        *dst[i] = cols[i] / 4;
+    }
+    if (require_device()) return 1;
+    if (pixie::gaussian_checkpoint_decode(table, n, row_words, c, K, has_threshold, threshold, pos, shs, opacity, cov, m_host, (cudaStream_t)stream))
+        return set_err("gaussian_checkpoint_decode failed");
     return 0;
 }
 // n^3 cells and their offsets are int32 on the device

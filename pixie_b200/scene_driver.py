@@ -31,7 +31,7 @@ from typing import Callable, Dict, Iterable, List, Optional, Sequence
 import numpy as np
 import torch
 
-from . import dist_utils, frame_export, gs_render, material_transfer, particle_filling, voxel_io
+from . import dist_utils, frame_export, gs_render, material_transfer, particle_filling, scene_files, voxel_io
 from .inference import MaterialFieldPredictor
 from .mpm_solver_warp import MPM_Simulator_WARP
 
@@ -77,6 +77,40 @@ class Scene:
     # frame positions; off, the solver's positions (the covariances stay in the Gaussians' frame either way)
     save_ply: bool = False
     to_original_coord: bool = True
+    # --optimization_output_path (gs_simulation.py:508-530): per-particle Young's moduli that replace the material field's
+    # after the hand-off (one per simulated particle, filled ones included); None keeps the hand-off's
+    e_field: Optional[torch.Tensor] = None
+
+    @classmethod
+    def from_files(cls, name: str, model_path: str, config: str, sh_degree: int = 3, iteration: int = -1, white_bg: bool = False,
+                   save_ply: bool = False, device="cuda:0", grid=None, mask=None, min_bounds=None, max_bounds=None) -> "Scene":
+        """The scene gs_simulation.py sets up (:355-437, :491-501) from a trained model directory and a physics config:
+        the checkpoint decoded on the device and filtered by the config's opacity_threshold, the config's rotations,
+        sim_area, particle_filling, camera keys, to_original_coord, fix_ground / only_handle_largest_cluster / k / nn
+        threshold and z shift, the model's cameras.json, and the material field's ground and stationary-cluster BCs,
+        which the reference always applies. `grid` / `mask` / bounds are only needed to take the neural path
+        (`SceneBatchDriver.run`). A config whose particle filling asks for `smooth` raises NotImplementedError before any
+        device work."""
+        mp, bc, tp, pp, cp = scene_files.decode_param_json(config)
+        check_supported(name, pp)
+        g = scene_files.load_gaussians(model_path, pp["opacity_threshold"], sh_degree, iteration, device)
+        return cls(name=name, grid=grid, mask=mask, min_bounds=min_bounds, max_bounds=max_bounds, particles=g["pos"], cov=g["cov3D_precomp"],
+                   material_params=mp, bc_params=list(bc), time_params=tp,
+                   rotation_matrices=scene_files.generate_rotation_matrices(pp["rotation_degree"], pp["rotation_axis"], device),
+                   z_shift_value=pp["z_shift_value"], k_smoothing_neighbors=pp["k_smoothing_neighbors"],
+                   nn_distance_threshold=pp["nn_distance_threshold"], material_field_bcs=True, fix_ground=pp["fix_ground"],
+                   only_handle_largest_cluster=pp["only_handle_largest_cluster"], opacity=g["opacity"], particle_filling=pp["particle_filling"],
+                   sim_area=pp["sim_area"], shs=g["shs"], sh_degree=sh_degree, camera_params=cp,
+                   cameras=os.path.join(model_path, "cameras.json"), white_bg=white_bg, save_ply=save_ply,
+                   to_original_coord=pp["to_original_coord"])
+
+
+def check_supported(name: str, preprocessing_params: Dict):
+    """Raises NotImplementedError for a config this package cannot simulate: particle filling with `smooth`, which needs
+    PyMCubes' constrained smoothing."""
+    pf = preprocessing_params.get("particle_filling")
+    if pf and pf.get("smooth", False):
+        raise NotImplementedError(f"scene {name}: particle filling with smooth needs mcubes.smooth (PyMCubes), which is not available")
 
 
 def transform2origin(position_tensor: torch.Tensor):
@@ -131,6 +165,14 @@ class SceneBatchDriver:
             self.predictor.load_state_dicts(seg_state_dict, cont_state_dict)
         self.ranges = ranges
         self.grid_size = grid_size
+
+    @classmethod
+    def physics_only(cls, device="cuda:0") -> "SceneBatchDriver":
+        """A driver for scenes whose material point cloud is already at hand (gs_simulation.py's --point_cloud_path): no
+        networks are built, so only run_physics_simulation is available."""
+        self = cls.__new__(cls)
+        self.device, self.predictor, self.ranges, self.grid_size = torch.device(device), None, None, None
+        return self
 
     # ------------------------------------------------------------------------------ neural half
     def generate_neural_segmentation(self, scenes: Sequence[Scene], out_dir: Optional[str] = None) -> List[Dict[str, torch.Tensor]]:
@@ -233,6 +275,12 @@ class SceneBatchDriver:
             props = material_transfer.perform_knn_smoothing(q, cloud, sc.k_smoothing_neighbors, sc.nn_distance_threshold)
             material_transfer.apply_material_properties_to_solver(solver, props[1], props[2], props[3], props[4], device=str(dev),
                                                                   exact_box_semantics=False)
+        if sc.e_field is not None:                                                                  # gs_simulation.py:527-531
+            E = sc.e_field.detach().to(dev, torch.float32).reshape(-1).contiguous()
+            if E.numel() != solver.n_particles:
+                raise ValueError(f"scene {sc.name}: the E field has {E.numel()} values for {solver.n_particles} particles")
+            solver.mpm_model.E = E
+            solver.finalize_mu_lam()
         substep_dt = tp["substep_dt"]
         step_per_frame = int(tp["frame_dt"] / substep_dt)                                           # float division like :627
         frames_pos, frames_cov, frames_rgb = [], [], []

@@ -51,6 +51,13 @@ def load_mask(path: str) -> torch.Tensor:
     return torch.from_numpy(np.load(path).astype(np.float32))
 
 
+def load_grid_metadata(npz_path: str) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """(min_bounds, max_bounds, grid_shape) of clip_features.npz, as map_pred_to_coords.py:146-150 reads them: the
+    bounds a Scene needs to place its predicted material field."""
+    with np.load(npz_path) as metadata:
+        return metadata["min_bounds"], metadata["max_bounds"], metadata["grid_shape"]
+
+
 class SceneGrid:
     """One scene of `scene_stream`: `.dir`, the pinned `.tensor`, and `.h2d_done` — the CUDA event after which the pinned
     buffer may be rewritten (set by the consumer, e.g. MaterialFieldPredictor.predict_packed_host_stream)."""
