@@ -148,6 +148,20 @@ int pixie_gaussian_ply_records(const float* pos_dev, const float* cov_dev, const
 int pixie_gaussian_checkpoint_decode(const void* table_dev, long long n, int row_bytes, const int* cols, int K, int has_threshold,
                                      float threshold, float* pos_dev, float* shs_dev, float* opacity_dev, float* cov_dev,
                                      long long* m_host, void* stream);
+/* pixie_material_metrics: the evaluation of the material networks on labelled scenes, process_batch's metric code
+ * (WG/trainer/inference_combined.py:108-170, compute_accuracy / masked_mean of pixie/training_utils.py:68-87) together with
+ * the ground-truth normalisation of MaterialVoxelDataset.__getitem__ (WG/data_utils/my_data.py:160-240).
+ * mat_dev [n][voxels][c_mat] fp32: material_grid.npy as it is on disk (channels-last; density, E, nu, ..., id last).
+ * mask_dev [n][voxels] fp32 (clip_features_mask.npy) or NULL, in which case the mask is (trunc(id) != background_id).
+ * seg_dev [n][n_classes][voxels] logits, cont_dev [n][3][voxels]. ranges (host) = {density_min, density_max, E_min, E_max,
+ * nu_min, nu_max} (log10 space for density and E). Outputs, device: gt_dev [n][4][voxels] = save_predictions' mat_grid
+ * (density, E: 2 (clip(log10(x + 1e-6), lo, hi) - lo) / (hi - lo) - 1; nu the same without the log; id as float(int64(id)));
+ * counts_dev [n][2] = (#(mask != 0), #(argmax == id & mask != 0)), torch.argmax rules (first index, NaN is the maximum);
+ * sums_dev [n][4] = (sum (cont_c - gt_c)^2 * mask for c = 0..2, sum mask), fp64 in a fixed order (bit-identical on a
+ * repeat). Stream-ordered, no host sync. */
+int pixie_material_metrics(const float* mat_dev, int c_mat, const float* mask_dev, const float* seg_dev, int n_classes, const float* cont_dev,
+                           int n, int64_t voxels, const double ranges[6], int background_id, float* gt_dev, long long* counts_dev,
+                           double* sums_dev, void* stream);
 /* ---- particle filling of hollow Gaussian objects (PG/particle_filling/filling.py:26-380, Taichi in the reference).
  * pixie_fill_density: densify_grids (:26-87). count_dev [grid_n^3] int32 = Gaussians per cell (a Gaussian outside the grid
  * counts in the nearest border cell; the reference indexes out of range), density_dev [grid_n^3] fp32 = sum over the

@@ -98,6 +98,8 @@ _SIGNATURES = {
     "pixie_gaussian_ply_records": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "pixie_gaussian_checkpoint_decode": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_float, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong), C.c_void_p]),
+    "pixie_material_metrics": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int64, C.POINTER(C.c_double),
+                                         C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pixie_fill_density": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pixie_fill_grids": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_float), C.c_float, C.c_float, C.c_int, C.c_int,
                                    C.c_int, C.c_ulonglong, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),

@@ -10,6 +10,7 @@
 #include "gs_render.cuh"
 #include "gs_ply.cuh"
 #include "gs_load.cuh"
+#include "material_metrics.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -178,6 +179,24 @@ int pixie_gaussian_checkpoint_decode(const void* table, long long n, int row_byt
     if (require_device()) return 1;
     if (pixie::gaussian_checkpoint_decode(table, n, row_words, c, K, has_threshold, threshold, pos, shs, opacity, cov, m_host, (cudaStream_t)stream))
         return set_err("gaussian_checkpoint_decode failed");
+    return 0;
+}
+int pixie_material_metrics(const float* mat, int c_mat, const float* mask, const float* seg, int n_classes, const float* cont, int n,
+                           int64_t voxels, const double* ranges, int background_id, float* gt, long long* counts, double* sums, void* stream) {
+    if (!ranges || (n > 0 && (!mat || !seg || !cont || !gt || !counts || !sums))) return set_err("null argument");
+    if (n < 0 || voxels < 1) return set_err("material_metrics: need n >= 0 samples of at least one voxel");
+    if (c_mat < 4) return set_err("material_metrics: the material grid needs at least 4 channels (density, E, nu, ..., material id)");
+    if (n_classes < 1) return set_err("material_metrics: need at least one class");
+    pixie::MaterialNorm nm;
+    for (int c = 0; c < 3; ++c) {
+        const double lo = ranges[2 * c], hi = ranges[2 * c + 1];
+        nm.lo[c] = (float)lo;
+        nm.hi[c] = (float)hi;
+        nm.span[c] = (float)(hi - lo);
+    }
+    if (require_device()) return 1;
+    if (pixie::material_metrics(mat, c_mat, mask, seg, n_classes, cont, n, voxels, nm, background_id, gt, counts, sums, (cudaStream_t)stream))
+        return set_err("material_metrics failed");
     return 0;
 }
 // n^3 cells and their offsets are int32 on the device
