@@ -116,7 +116,7 @@ int pixie_cluster_stats(const float* pos_dev, const int* index_dev, const int* l
 /* ---- either side of the substep loop (SURVEY.md 8f-2).
  * pixie_particle_volume: get_particle_volume, PG/particle_filling/filling.py:247-288 (Taichi in the reference): particles per cell
  * of a grid_n^3 grid of spacing grid_dx, vol = grid_dx^3 / count. Positions outside the grid are clamped to the border cells
- * (the reference indexes out of range). Synchronises `stream`. */
+ * (the reference indexes out of range). Stream-ordered, no host sync. */
 int pixie_particle_volume(const float* pos_dev, int n, int grid_n, float grid_dx, float* vol_dev, void* stream);
 /* pixie_frame_transform: per-frame hand-over to the rasteriser, gs_simulation.py:591-600 with utils/transformation_utils.py:19-20,
  * 57-87, 101-126: pos_render = apply_inverse_rotations(mean + (pos - (1,1,1+z_shift)) / scale, Rs); cov_render =

@@ -19,6 +19,8 @@
 namespace {
 thread_local std::string g_err;
 int set_err(const std::string& e) { g_err = e; return 1; }
+// 0 on success, otherwise 1 with "<op>: <CUDA's description of e>" as the last error
+int check(const char* op, cudaError_t e) { return e == cudaSuccess ? 0 : set_err(std::string(op) + ": " + cudaGetErrorString(e)); }
 }  // namespace
 
 struct pixie_unet_s { pixie::UNet* u; };
@@ -87,11 +89,11 @@ int pixie_unet_profile(pixie_unet_t h, const void* feat, int batch, float* out, 
 int pixie_field_extract(const float* pred, int n_classes, const float* mask, int D, const double ranges[6], const double bmin[3], const double bmax[3],
                         float* pos, float* density, float* E, float* nu, int* material, float* conf, int* count_host, void* stream) {
     if (!pred || !mask || !ranges || !bmin || !bmax || !pos || !density || !E || !nu || !material || !conf || !count_host) return set_err("null argument");
-    if (D < 2 || n_classes < 1) return set_err("field_extract: need D >= 2 and at least one class channel");
+    if (D < 2 || D > 1290 || n_classes < 1)
+        return set_err("field_extract: need 2 <= D <= 1290 (D^3 voxels are indexed in int32) and at least one class channel");
     if (require_device()) return 1;
-    if (pixie::field_extract(pred, n_classes, mask, D, ranges, bmin, bmax, pos, density, E, nu, material, conf, count_host, (cudaStream_t)stream))
-        return set_err("field_extract failed");
-    return 0;
+    return check("field_extract", pixie::field_extract(pred, n_classes, mask, D, ranges, bmin, bmax, pos, density, E, nu, material, conf,
+                                                       count_host, (cudaStream_t)stream));
 }
 int pixie_knn_assign(const float* query, int nq, const float* pos, const float* density, const float* E, const float* nu, const int* material,
                      const int* part, const float* conf, int m, int k, double threshold, int weighted, const float defaults[4], int def_material,
@@ -103,10 +105,9 @@ int pixie_knn_assign(const float* query, int nq, const float* pos, const float* 
     if (m < 1) return set_err("knn_assign: empty material point cloud");
     if (k > m) return set_err("knn_assign: k exceeds the number of material points");
     if (require_device()) return 1;
-    if (pixie::knn_assign(query, nq, pos, density, E, nu, material, part, conf, m, k, threshold, weighted, defaults, def_material, def_part,
-                          o_density, o_E, o_nu, o_material, o_part, o_conf, n_too_far_host, (cudaStream_t)stream))
-        return set_err("knn_assign failed");
-    return 0;
+    return check("knn_assign", pixie::knn_assign(query, nq, pos, density, E, nu, material, part, conf, m, k, threshold, weighted, defaults,
+                                                 def_material, def_part, o_density, o_E, o_nu, o_material, o_part, o_conf, n_too_far_host,
+                                                 (cudaStream_t)stream));
 }
 int pixie_dbscan(const float* pos, int n, const int* ids, int select_id, double eps, int min_samples, int* index, int* labels,
                  int* n_selected_host, int* n_clusters_host, void* stream) {
@@ -114,26 +115,22 @@ int pixie_dbscan(const float* pos, int n, const int* ids, int select_id, double 
     if (n < 0) return set_err("dbscan: negative point count");
     if (!(eps > 0.0) || min_samples < 1) return set_err("dbscan: need eps > 0 and min_samples >= 1");
     if (require_device()) return 1;
-    if (pixie::dbscan(pos, n, ids, select_id, eps, min_samples, index, labels, n_selected_host, n_clusters_host, (cudaStream_t)stream))
-        return set_err("dbscan failed");
-    return 0;
+    return check("dbscan", pixie::dbscan(pos, n, ids, select_id, eps, min_samples, index, labels, n_selected_host, n_clusters_host,
+                                         (cudaStream_t)stream));
 }
 int pixie_cluster_stats(const float* pos, const int* index, const int* labels, int n_selected, int n_clusters, int* sizes,
                         float* bbox_min, float* bbox_max, void* stream) {
     if (n_selected < 0 || n_clusters < 0) return set_err("cluster_stats: negative count");
     if ((n_selected > 0 && (!pos || !index || !labels)) || (n_clusters > 0 && (!sizes || !bbox_min || !bbox_max))) return set_err("null argument");
     if (require_device()) return 1;
-    if (pixie::cluster_stats(pos, index, labels, n_selected, n_clusters, sizes, bbox_min, bbox_max, (cudaStream_t)stream))
-        return set_err("cluster_stats failed");
-    return 0;
+    return check("cluster_stats", pixie::cluster_stats(pos, index, labels, n_selected, n_clusters, sizes, bbox_min, bbox_max, (cudaStream_t)stream));
 }
 int pixie_particle_volume(const float* pos, int n, int grid_n, float grid_dx, float* vol, void* stream) {
     if (n < 0) return set_err("particle_volume: negative point count");
     if (n > 0 && (!pos || !vol)) return set_err("null argument");
     if (grid_n < 1 || !(grid_dx > 0.f)) return set_err("particle_volume: bad grid");
     if (require_device()) return 1;
-    if (pixie::particle_volume(pos, n, grid_n, grid_dx, vol, (cudaStream_t)stream)) return set_err("particle_volume failed");
-    return 0;
+    return check("particle_volume", pixie::particle_volume(pos, n, grid_n, grid_dx, vol, (cudaStream_t)stream));
 }
 int pixie_frame_transform(const float* pos, const float* cov, int n, float z_shift, float scale, const float mean[3], const float* rotations,
                           int n_rot, float* pos_out, float* cov_out, void* stream) {
@@ -141,8 +138,7 @@ int pixie_frame_transform(const float* pos, const float* cov, int n, float z_shi
     if (!mean || (n > 0 && (!pos || !pos_out || (cov && !cov_out))) || (n_rot > 0 && !rotations)) return set_err("null argument");
     if (n_rot < 0 || n_rot > 8) return set_err("frame_transform: at most 8 rotations");
     if (require_device()) return 1;
-    if (pixie::frame_transform(pos, cov, n, z_shift, scale, mean, rotations, n_rot, pos_out, cov_out, (cudaStream_t)stream)) return set_err("frame_transform failed");
-    return 0;
+    return check("frame_transform", pixie::frame_transform(pos, cov, n, z_shift, scale, mean, rotations, n_rot, pos_out, cov_out, (cudaStream_t)stream));
 }
 int pixie_gaussian_ply_records(const float* pos, const float* cov, const float* shs, int K, const float* opacity, int n, float* records,
                                void* stream) {
@@ -150,8 +146,7 @@ int pixie_gaussian_ply_records(const float* pos, const float* cov, const float* 
     if (K != 1 && K != 4 && K != 9 && K != 16) return set_err("gaussian_ply_records: K must be 1, 4, 9 or 16 SH coefficients");
     if (n > 0 && (!pos || !cov || !shs || !opacity || !records)) return set_err("null argument");
     if (require_device()) return 1;
-    if (pixie::gaussian_ply_records(pos, cov, shs, K, opacity, n, records, (cudaStream_t)stream)) return set_err("gaussian_ply_records failed");
-    return 0;
+    return check("gaussian_ply_records", pixie::gaussian_ply_records(pos, cov, shs, K, opacity, n, records, (cudaStream_t)stream));
 }
 int pixie_gaussian_checkpoint_decode(const void* table, long long n, int row_bytes, const int* cols, int K, int has_threshold, float threshold,
                                      float* pos, float* shs, float* opacity, float* cov, long long* m_host, void* stream) {
@@ -177,9 +172,8 @@ int pixie_gaussian_checkpoint_decode(const void* table, long long n, int row_byt
         *dst[i] = cols[i] / 4;
     }
     if (require_device()) return 1;
-    if (pixie::gaussian_checkpoint_decode(table, n, row_words, c, K, has_threshold, threshold, pos, shs, opacity, cov, m_host, (cudaStream_t)stream))
-        return set_err("gaussian_checkpoint_decode failed");
-    return 0;
+    return check("gaussian_checkpoint_decode", pixie::gaussian_checkpoint_decode(table, n, row_words, c, K, has_threshold, threshold, pos, shs, opacity,
+                                                                                 cov, m_host, (cudaStream_t)stream));
 }
 int pixie_material_metrics(const float* mat, int c_mat, const float* mask, const float* seg, int n_classes, const float* cont, int n,
                            int64_t voxels, const double* ranges, int background_id, float* gt, long long* counts, double* sums, void* stream) {
@@ -195,9 +189,8 @@ int pixie_material_metrics(const float* mat, int c_mat, const float* mask, const
         nm.span[c] = (float)(hi - lo);
     }
     if (require_device()) return 1;
-    if (pixie::material_metrics(mat, c_mat, mask, seg, n_classes, cont, n, voxels, nm, background_id, gt, counts, sums, (cudaStream_t)stream))
-        return set_err("material_metrics failed");
-    return 0;
+    return check("material_metrics", pixie::material_metrics(mat, c_mat, mask, seg, n_classes, cont, n, voxels, nm, background_id, gt, counts, sums,
+                                                             (cudaStream_t)stream));
 }
 // n^3 cells and their offsets are int32 on the device
 static bool fill_grid_ok(int grid_n) { return grid_n >= 1 && grid_n <= 1290; }
@@ -206,8 +199,7 @@ int pixie_fill_density(const float* pos, const float* opacity, const float* cov,
     if (!count || !density || (n > 0 && (!pos || !opacity || !cov))) return set_err("null argument");
     if (n < 0 || !fill_grid_ok(grid_n) || !(grid_dx > 0.f)) return set_err("fill_density: need n >= 0, 1 <= grid_n <= 1290 and grid_dx > 0");
     if (require_device()) return 1;
-    if (pixie::fill_density(pos, opacity, cov, n, grid_n, grid_dx, count, density, (cudaStream_t)stream)) return set_err("fill_density failed");
-    return 0;
+    return check("fill_density", pixie::fill_density(pos, opacity, cov, n, grid_n, grid_dx, count, density, (cudaStream_t)stream));
 }
 int pixie_fill_grids(int* count, const float* density, int grid_n, float grid_dx, const float origin[3], float density_thres, float search_thres,
                      int max_particles_per_cell, int exclude_dir, int ray_cast_dir, unsigned long long seed, float* out, int max_samples,
@@ -219,20 +211,19 @@ int pixie_fill_grids(int* count, const float* density, int grid_n, float grid_dx
     if (exclude_dir < 0 || exclude_dir > 5 || ray_cast_dir < 0 || ray_cast_dir > 5) return set_err("fill_grids: directions must be in 0..5");
     if (max_samples < 0) return set_err("fill_grids: negative max_samples");
     if (require_device()) return 1;
-    const int rc = pixie::fill_grids(count, density, grid_n, grid_dx, origin, density_thres, search_thres, max_particles_per_cell, exclude_dir,
-                                     ray_cast_dir, seed, out, max_samples, n_dense_host, n_total_host, (cudaStream_t)stream);
-    if (rc == 3)
+    if (check("fill_grids", pixie::fill_grids(count, density, grid_n, grid_dx, origin, density_thres, search_thres, max_particles_per_cell,
+                                              exclude_dir, ray_cast_dir, seed, out, max_samples, n_dense_host, n_total_host, (cudaStream_t)stream)))
+        return 1;
+    if (*n_total_host > max_samples)
         return set_err("fill_grids: filling adds " + std::to_string(*n_total_host) + " particles (" + std::to_string(*n_dense_host) +
                        " in dense cells) but max_samples is " + std::to_string(max_samples));
-    if (rc) return set_err("fill_grids failed");
     return 0;
 }
 int pixie_nearest_gaussian(const float* pos, int n, const float* query, int m, int* index, void* stream) {
     if (n < 0 || m < 0) return set_err("nearest_gaussian: negative count");
     if ((n > 0 && m > 0 && !pos) || (m > 0 && (!query || !index))) return set_err("null argument");
     if (require_device()) return 1;
-    if (pixie::nearest_gaussian(pos, n, query, m, index, (cudaStream_t)stream)) return set_err("nearest_gaussian failed");
-    return 0;
+    return check("nearest_gaussian", pixie::nearest_gaussian(pos, n, query, m, index, (cudaStream_t)stream));
 }
 // ------------------------------------------------------------------------------------- Gaussian rasteriser
 int pixie_gs_renderer_create(pixie_gs_renderer_t* out) {
@@ -274,8 +265,8 @@ void pixie_gs_renderer_destroy(pixie_gs_renderer_t h) {
 int pixie_pack_predictions(const float* seg_logits_dev, const float* cont_dev, float* out_dev, int batch, int64_t voxels, int n_classes, void* stream) {
     if (!seg_logits_dev || !cont_dev || !out_dev) return set_err("null argument");
     if (require_device()) return 1;
-    if (pixie::launch_pack_predictions(seg_logits_dev, cont_dev, out_dev, batch, voxels, n_classes, (cudaStream_t)stream)) return set_err("launch failed");
-    return 0;
+    return check("pack_predictions",
+                 (cudaError_t)pixie::launch_pack_predictions(seg_logits_dev, cont_dev, out_dev, batch, voxels, n_classes, (cudaStream_t)stream));
 }
 int pixie_unet_launch_count(pixie_unet_t h) { return h ? pixie::unet_launch_count(h->u) : 0; }
 double pixie_unet_flops(pixie_unet_t h) { return h ? pixie::unet_flops(h->u) : 0.0; }
@@ -362,7 +353,10 @@ int pixie_ipc_open(const unsigned char handle[64], void** dev_ptr) {
         return set_err(std::string("cudaIpcOpenMemHandle: ") + cudaGetErrorString(cudaGetLastError()));
     return 0;
 }
-int pixie_ipc_close(void* dev_ptr) { return cudaIpcCloseMemHandle(dev_ptr) == cudaSuccess ? 0 : set_err("cudaIpcCloseMemHandle failed"); }
+int pixie_ipc_close(void* dev_ptr) {
+    if (cudaIpcCloseMemHandle(dev_ptr) != cudaSuccess) return set_err(std::string("cudaIpcCloseMemHandle: ") + cudaGetErrorString(cudaGetLastError()));
+    return 0;
+}
 long long pixie_mpm_launch_count(pixie_mpm_t h) { return h ? pixie::mpm_launch_count(h->m) : 0; }
 void pixie_mpm_destroy(pixie_mpm_t h) {
     if (!h) return;

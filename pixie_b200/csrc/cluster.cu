@@ -20,6 +20,7 @@
 //                  the exclusive scan of the root flags.
 //   5. borders     minimum label over the core neighbours.
 #include "cluster.cuh"
+#include "workspace.cuh"
 
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
@@ -263,31 +264,21 @@ __global__ void decode_kernel(unsigned* __restrict__ a, unsigned* __restrict__ b
     }
 }
 
-struct Workspace {
-    void* base = nullptr;
-    size_t off = 0;
-    template <class T> T* take(size_t count) {
-        T* p = reinterpret_cast<T*>(static_cast<char*>(base) + off);
-        off += (count * sizeof(T) + 255) & ~size_t(255);
-        return p;
-    }
-};
-
 }  // namespace
 
-int dbscan(const float* pos, int n, const int* ids, int select_id, double eps, int min_samples, int* index, int* labels,
-           int* n_selected_host, int* n_clusters_host, cudaStream_t st) {
-    if (n <= 0) { *n_selected_host = 0; *n_clusters_host = 0; return 0; }
+cudaError_t dbscan(const float* pos, int n, const int* ids, int select_id, double eps, int min_samples, int* index, int* labels,
+                   int* n_selected_host, int* n_clusters_host, cudaStream_t st) {
+    if (n <= 0) { *n_selected_host = 0; *n_clusters_host = 0; return cudaSuccess; }
     const size_t N = (size_t)n;
     // sizes of every cub call, then one allocation for everything
     size_t tb[5] = {0, 0, 0, 0, 0};
     thrust::counting_iterator<int> iota(0);
-    cub::DeviceSelect::Flagged(nullptr, tb[0], iota, (const int*)nullptr, (int*)nullptr, (int*)nullptr, n, st);
-    cub::DeviceRadixSort::SortPairs(nullptr, tb[1], (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (const int*)nullptr,
-                                    (int*)nullptr, n, 0, 64, st);
-    cub::DeviceRunLengthEncode::Encode(nullptr, tb[2], (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr,
-                                       (int*)nullptr, n, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, tb[3], (const int*)nullptr, (int*)nullptr, n + 1, st);
+    PIXIE_TRY(cub::DeviceSelect::Flagged(nullptr, tb[0], iota, (const int*)nullptr, (int*)nullptr, (int*)nullptr, n, st));
+    PIXIE_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb[1], (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                              (const int*)nullptr, (int*)nullptr, n, 0, 64, st));
+    PIXIE_TRY(cub::DeviceRunLengthEncode::Encode(nullptr, tb[2], (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                                 (int*)nullptr, (int*)nullptr, n, st));
+    PIXIE_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb[3], (const int*)nullptr, (int*)nullptr, n + 1, st));
     size_t tmp_bytes = 0;
     for (size_t b : tb) tmp_bytes = b > tmp_bytes ? b : tmp_bytes;
     int *counts, *n_runs, *flags, *vals_in, *order, *run_len, *start, *parent, *root_flag, *root_rank;   // counts = {M, n_clusters}
@@ -296,61 +287,55 @@ int dbscan(const float* pos, int n, const int* ids, int select_id, double eps, i
     unsigned long long *keys_in, *keys, *uniq;
     float4* sp;
     uint8_t *core_s, *core_t;
-    auto carve = [&](Workspace& w) {
+    Workspace w(st);
+    PIXIE_TRY(w.carve([&] {
         counts = w.take<int>(2); mn = w.take<unsigned>(3); n_runs = w.take<int>(1); tmp = w.take<char>(tmp_bytes);
         flags = w.take<int>(N); keys_in = w.take<unsigned long long>(N); keys = w.take<unsigned long long>(N);
         uniq = w.take<unsigned long long>(N); vals_in = w.take<int>(N); order = w.take<int>(N); run_len = w.take<int>(N + 1);
         start = w.take<int>(N + 1); sp = w.take<float4>(N); core_s = w.take<uint8_t>(N); core_t = w.take<uint8_t>(N);
         parent = w.take<int>(N); root_flag = w.take<int>(N + 1); root_rank = w.take<int>(N + 1);
-    };
-    Workspace sizing;
-    carve(sizing);
-    Workspace w;
-    if (cudaMalloc(&w.base, sizing.off) != cudaSuccess) return 1;
-    carve(w);
+    }));
 
     const int B = 256, G = (int)((N + B - 1) / B);
     const double cell = eps * (1.0 + 1e-6);
-    cudaMemsetAsync(mn, 0xff, 3 * sizeof(unsigned), st);
-    cudaMemsetAsync(run_len, 0, (N + 1) * sizeof(int), st);
-    cudaMemsetAsync(root_flag, 0, (N + 1) * sizeof(int), st);
+    PIXIE_TRY(cudaMemsetAsync(mn, 0xff, 3 * sizeof(unsigned), st));
+    PIXIE_TRY(cudaMemsetAsync(run_len, 0, (N + 1) * sizeof(int), st));
+    PIXIE_TRY(cudaMemsetAsync(root_flag, 0, (N + 1) * sizeof(int), st));
     flag_kernel<<<G, B, 0, st>>>(ids, n, select_id, flags);
-    cub::DeviceSelect::Flagged(tmp, tb[0], iota, flags, index, counts, n, st);
+    PIXIE_TRY(cub::DeviceSelect::Flagged(tmp, tb[0], iota, flags, index, counts, n, st));
     min_corner_kernel<<<G, B, 0, st>>>(pos, index, counts, n, mn);
     key_kernel<<<G, B, 0, st>>>(pos, index, counts, n, mn, cell, keys_in, vals_in);
-    cub::DeviceRadixSort::SortPairs(tmp, tb[1], keys_in, keys, vals_in, order, n, 0, 64, st);
-    cub::DeviceRunLengthEncode::Encode(tmp, tb[2], keys, uniq, run_len, n_runs, n, st);
-    cub::DeviceScan::ExclusiveSum(tmp, tb[3], run_len, start, n + 1, st);
+    PIXIE_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb[1], keys_in, keys, vals_in, order, n, 0, 64, st));
+    PIXIE_TRY(cub::DeviceRunLengthEncode::Encode(tmp, tb[2], keys, uniq, run_len, n_runs, n, st));
+    PIXIE_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb[3], run_len, start, n + 1, st));
     gather_kernel<<<G, B, 0, st>>>(pos, index, counts, n, order, sp);
     Grid g{sp, uniq, start, n_runs, counts, eps * eps};
     core_kernel<<<G, B, 0, st>>>(g, keys, n, min_samples, core_s, core_t, parent);
     union_kernel<<<G, B, 0, st>>>(g, keys, n, core_s, parent);
     root_kernel<<<G, B, 0, st>>>(counts, n, core_t, parent, root_flag);
-    cub::DeviceScan::ExclusiveSum(tmp, tb[3], root_flag, root_rank, n + 1, st);
+    PIXIE_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb[3], root_flag, root_rank, n + 1, st));
     label_kernel<<<G, B, 0, st>>>(counts, n, core_t, parent, root_rank, labels);
     border_kernel<<<G, B, 0, st>>>(g, keys, n, core_s, labels);
-    cudaMemcpyAsync(counts + 1, root_rank + N, sizeof(int), cudaMemcpyDeviceToDevice, st);
+    PIXIE_TRY(cudaMemcpyAsync(counts + 1, root_rank + N, sizeof(int), cudaMemcpyDeviceToDevice, st));
     int host[2] = {0, 0};
-    int rc = cudaMemcpyAsync(host, counts, 2 * sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess;
-    rc |= cudaStreamSynchronize(st) != cudaSuccess;
-    rc |= cudaGetLastError() != cudaSuccess;
-    cudaFree(w.base);
+    PIXIE_TRY(cudaMemcpyAsync(host, counts, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    PIXIE_TRY(cudaStreamSynchronize(st));
     *n_selected_host = host[0];
     *n_clusters_host = host[1];
-    return rc;
+    return cudaGetLastError();
 }
 
-int cluster_stats(const float* pos, const int* index, const int* labels, int n_selected, int n_clusters, int* sizes,
-                  float* bbox_min, float* bbox_max, cudaStream_t st) {
-    if (n_clusters <= 0) return 0;
-    cudaMemsetAsync(sizes, 0, (size_t)n_clusters * sizeof(int), st);
-    cudaMemsetAsync(bbox_min, 0xff, (size_t)n_clusters * 3 * sizeof(float), st);     // encoded +max
-    cudaMemsetAsync(bbox_max, 0, (size_t)n_clusters * 3 * sizeof(float), st);        // encoded -max
+cudaError_t cluster_stats(const float* pos, const int* index, const int* labels, int n_selected, int n_clusters, int* sizes,
+                          float* bbox_min, float* bbox_max, cudaStream_t st) {
+    if (n_clusters <= 0) return cudaSuccess;
+    PIXIE_TRY(cudaMemsetAsync(sizes, 0, (size_t)n_clusters * sizeof(int), st));
+    PIXIE_TRY(cudaMemsetAsync(bbox_min, 0xff, (size_t)n_clusters * 3 * sizeof(float), st));     // encoded +max
+    PIXIE_TRY(cudaMemsetAsync(bbox_max, 0, (size_t)n_clusters * 3 * sizeof(float), st));        // encoded -max
     unsigned* lo = reinterpret_cast<unsigned*>(bbox_min);
     unsigned* hi = reinterpret_cast<unsigned*>(bbox_max);
     if (n_selected > 0) stats_kernel<<<(n_selected + 255) / 256, 256, 0, st>>>(pos, index, labels, n_selected, sizes, lo, hi);
     decode_kernel<<<(3 * n_clusters + 255) / 256, 256, 0, st>>>(lo, hi, 3 * n_clusters);
-    return cudaGetLastError() != cudaSuccess;
+    return cudaGetLastError();
 }
 
 }  // namespace pixie

@@ -6,6 +6,7 @@
 //                   neighbours (brute force, shared-memory tiles, distances in fp64 like sklearn's KDTree), mean / mode
 //                   of the neighbours' properties, defaults for particles farther than the threshold.
 #include "field_transfer.cuh"
+#include "workspace.cuh"
 
 #include <cub/cub.cuh>
 
@@ -257,68 +258,62 @@ __global__ void frame_transform_kernel(const FrameArgs a) {
 
 }  // namespace
 
-int field_extract(const float* pred, int n_classes, const float* mask, int D, const double ranges[6], const double bmin[3], const double bmax[3],
-                  float* pos, float* density, float* E, float* nu, int* material, float* conf, int* count_host, cudaStream_t st) {
+cudaError_t field_extract(const float* pred, int n_classes, const float* mask, int D, const double ranges[6], const double bmin[3], const double bmax[3],
+                          float* pos, float* density, float* E, float* nu, int* material, float* conf, int* count_host, cudaStream_t st) {
     const int n = D * D * D;
     int *flags = nullptr, *offsets = nullptr;
     void* tmp = nullptr;
     size_t tmp_bytes = 0;
-    if (cudaMalloc(&flags, (size_t)(n + 1) * sizeof(int)) != cudaSuccess || cudaMalloc(&offsets, (size_t)(n + 1) * sizeof(int)) != cudaSuccess) {
-        cudaFree(flags); cudaFree(offsets); return 1;
-    }
-    cudaMemsetAsync(flags, 0, (size_t)(n + 1) * sizeof(int), st);
+    PIXIE_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flags, offsets, n + 1, st));
+    Workspace w(st);
+    PIXIE_TRY(w.carve([&] { flags = w.take<int>(n + 1); offsets = w.take<int>(n + 1); tmp = w.take<char>(tmp_bytes); }));
+    PIXIE_TRY(cudaMemsetAsync(flags, 0, (size_t)(n + 1) * sizeof(int), st));
     field_flag_kernel<<<(n + 255) / 256, 256, 0, st>>>(mask, n, flags);
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flags, offsets, n + 1, st);
-    if (cudaMalloc(&tmp, tmp_bytes) != cudaSuccess) { cudaFree(flags); cudaFree(offsets); return 1; }
-    cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flags, offsets, n + 1, st);
+    PIXIE_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flags, offsets, n + 1, st));
     ExtractArgs a{};
     a.pred = pred; a.mask = mask; a.offsets = offsets; a.D = D; a.K = n_classes;
     for (int c = 0; c < 3; ++c) { a.lo[c] = ranges[2 * c]; a.hi[c] = ranges[2 * c + 1]; a.bmin[c] = bmin[c]; a.bmax[c] = bmax[c]; }
     a.pos = pos; a.density = density; a.E = E; a.nu = nu; a.conf = conf; a.material = material;
     field_extract_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
-    int rc = cudaMemcpyAsync(count_host, offsets + n, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess;
-    rc |= cudaStreamSynchronize(st) != cudaSuccess;
-    cudaFree(tmp); cudaFree(flags); cudaFree(offsets);
-    return rc || cudaGetLastError() != cudaSuccess;
+    PIXIE_TRY(cudaMemcpyAsync(count_host, offsets + n, sizeof(int), cudaMemcpyDeviceToHost, st));
+    PIXIE_TRY(cudaStreamSynchronize(st));
+    return cudaGetLastError();
 }
 
-int knn_assign(const float* query, int nq, const float* pos, const float* density, const float* E, const float* nu, const int* material,
-               const int* part, const float* conf, int m, int k, double threshold, int weighted, const float defaults[4], int def_material,
-               int def_part, float* o_density, float* o_E, float* o_nu, int* o_material, int* o_part, float* o_conf, int* n_too_far_host,
-               cudaStream_t st) {
-    if (k < 1 || k > kKnnMaxK) return 2;
+cudaError_t knn_assign(const float* query, int nq, const float* pos, const float* density, const float* E, const float* nu, const int* material,
+                       const int* part, const float* conf, int m, int k, double threshold, int weighted, const float defaults[4], int def_material,
+                       int def_part, float* o_density, float* o_E, float* o_nu, int* o_material, int* o_part, float* o_conf, int* n_too_far_host,
+                       cudaStream_t st) {
+    Workspace w(st);
     int* d_cnt = nullptr;
-    if (cudaMalloc(&d_cnt, sizeof(int)) != cudaSuccess) return 1;
-    cudaMemsetAsync(d_cnt, 0, sizeof(int), st);
+    PIXIE_TRY(w.carve([&] { d_cnt = w.take<int>(1); }));
+    PIXIE_TRY(cudaMemsetAsync(d_cnt, 0, sizeof(int), st));
     KnnArgs a{};
     a.query = query; a.nq = nq; a.pos = pos; a.density = density; a.E = E; a.nu = nu; a.conf = conf; a.material = material; a.part = part; a.m = m;
     a.k = k; a.threshold = threshold; a.weighted = weighted;
     a.def_density = defaults[0]; a.def_E = defaults[1]; a.def_nu = defaults[2]; a.def_conf = defaults[3]; a.def_material = def_material; a.def_part = def_part;
     a.o_density = o_density; a.o_E = o_E; a.o_nu = o_nu; a.o_conf = o_conf; a.o_material = o_material; a.o_part = o_part; a.n_too_far = d_cnt;
     if (nq > 0) knn_assign_kernel<<<(nq + 127) / 128, 128, 0, st>>>(a);
-    int rc = cudaMemcpyAsync(n_too_far_host, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess;
-    rc |= cudaStreamSynchronize(st) != cudaSuccess;
-    cudaFree(d_cnt);
-    return rc || cudaGetLastError() != cudaSuccess;
+    PIXIE_TRY(cudaMemcpyAsync(n_too_far_host, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, st));
+    PIXIE_TRY(cudaStreamSynchronize(st));
+    return cudaGetLastError();
 }
 
-int particle_volume(const float* pos, int n, int grid_n, float grid_dx, float* vol, cudaStream_t st) {
-    int* grid = nullptr;
+cudaError_t particle_volume(const float* pos, int n, int grid_n, float grid_dx, float* vol, cudaStream_t st) {
     const size_t cells = (size_t)grid_n * grid_n * grid_n;
-    if (cudaMalloc(&grid, cells * sizeof(int)) != cudaSuccess) return 1;
-    cudaMemsetAsync(grid, 0, cells * sizeof(int), st);
+    Workspace w(st);
+    int* grid = nullptr;
+    PIXIE_TRY(w.carve([&] { grid = w.take<int>(cells); }));
+    PIXIE_TRY(cudaMemsetAsync(grid, 0, cells * sizeof(int), st));
     if (n > 0) {
         volume_count_kernel<<<(n + 255) / 256, 256, 0, st>>>(pos, n, grid_dx, grid_n, grid);
         volume_assign_kernel<<<(n + 255) / 256, 256, 0, st>>>(pos, n, grid_dx, grid_n, grid, vol);
     }
-    const int rc = cudaStreamSynchronize(st) != cudaSuccess;
-    cudaFree(grid);
-    return rc || cudaGetLastError() != cudaSuccess;
+    return cudaGetLastError();
 }
 
-int frame_transform(const float* pos, const float* cov, int n, float z_shift, float scale, const float mean[3], const float* rotations, int n_rot,
-                    float* pos_out, float* cov_out, cudaStream_t st) {
-    if (n_rot < 0 || n_rot > 8) return 2;
+cudaError_t frame_transform(const float* pos, const float* cov, int n, float z_shift, float scale, const float mean[3], const float* rotations, int n_rot,
+                            float* pos_out, float* cov_out, cudaStream_t st) {
     FrameArgs a{};
     a.pos = pos; a.cov = cov; a.n = n; a.z_shift = z_shift; a.scale = scale;
     for (int d = 0; d < 3; ++d) a.mean[d] = mean[d];
@@ -326,7 +321,7 @@ int frame_transform(const float* pos, const float* cov, int n, float z_shift, fl
         for (int i = 0; i < 9; ++i) a.R[r][i] = rotations[9 * r + i];
     a.n_rot = n_rot; a.pos_out = pos_out; a.cov_out = cov_out;
     if (n > 0) frame_transform_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
-    return cudaGetLastError() != cudaSuccess;
+    return cudaGetLastError();
 }
 
 }  // namespace pixie

@@ -13,6 +13,7 @@
 // With a threshold, a first pass counts each block's kept rows, cub scans the counts, and the decode pass writes the kept
 // rows at the block's offset plus their rank in the block (warp ballots), which keeps file order.
 #include "gs_load.cuh"
+#include "workspace.cuh"
 
 #include <cub/cub.cuh>
 #include <cstdint>
@@ -130,55 +131,46 @@ __global__ void __launch_bounds__(kRows) decode_kernel(const float* __restrict__
 }
 
 template <int K>
-int launch_decode(const float* table, long long n, int row_words, const GsColumns& cols, int has_threshold, float threshold,
-                  const long long* offsets, float* pos, float* shs, float* opacity, float* cov, cudaStream_t st) {
+cudaError_t launch_decode(const float* table, long long n, int row_words, const GsColumns& cols, int has_threshold, float threshold,
+                          const long long* offsets, float* pos, float* shs, float* opacity, float* cov, cudaStream_t st) {
     const size_t smem = (size_t)kRows * row_words * sizeof(float);
-    if (smem > 48 * 1024 &&
-        cudaFuncSetAttribute(decode_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-        return 1;
+    if (smem > 48 * 1024) PIXIE_TRY(cudaFuncSetAttribute(decode_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const long long blocks = (n + kRows - 1) / kRows;
     decode_kernel<K><<<(unsigned)blocks, kRows, smem, st>>>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs, opacity, cov);
-    return cudaGetLastError() != cudaSuccess;
+    return cudaGetLastError();
 }
 
 }  // namespace
 
-int gaussian_checkpoint_decode(const void* table_v, long long n, int row_words, const GsColumns& cols, int K, int has_threshold,
-                               float threshold, float* pos, float* shs, float* opacity, float* cov, long long* m_host, cudaStream_t st) {
-    if (K != 1 && K != 4 && K != 9 && K != 16) return 2;
-    if (row_words < 1 || row_words > kGsLoadMaxRowWords) return 2;
+cudaError_t gaussian_checkpoint_decode(const void* table_v, long long n, int row_words, const GsColumns& cols, int K, int has_threshold,
+                                       float threshold, float* pos, float* shs, float* opacity, float* cov, long long* m_host, cudaStream_t st) {
     *m_host = 0;
-    if (n <= 0) return 0;
+    if (n <= 0) return cudaSuccess;
     const float* table = static_cast<const float*>(table_v);
     const long long blocks = (n + kRows - 1) / kRows;
-    long long* counts = nullptr;           // [blocks + 1] counts, then [blocks + 1] offsets
-    void* tmp = nullptr;
-    size_t tmp_bytes = 0;
-    int rc = 0;
+    long long *counts = nullptr, *offsets = nullptr;      // [blocks + 1] each, with a threshold
+    Workspace w(st);
     if (has_threshold) {
-        if (cudaMallocAsync(&counts, 2 * (blocks + 1) * sizeof(long long), st) != cudaSuccess) return 1;
-        long long* offsets = counts + blocks + 1;
-        cudaMemsetAsync(counts + blocks, 0, sizeof(long long), st);
+        void* tmp = nullptr;
+        size_t tmp_bytes = 0;
+        PIXIE_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, counts, offsets, (int)(blocks + 1), st));
+        PIXIE_TRY(w.carve([&] { counts = w.take<long long>(blocks + 1); offsets = w.take<long long>(blocks + 1); tmp = w.take<char>(tmp_bytes); }));
+        PIXIE_TRY(cudaMemsetAsync(counts + blocks, 0, sizeof(long long), st));
         count_kernel<<<(unsigned)blocks, kRows, 0, st>>>(table, n, row_words, cols.opacity, threshold, counts);
-        cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, counts, offsets, (int)(blocks + 1), st);
-        rc |= cudaMallocAsync(&tmp, tmp_bytes, st) != cudaSuccess;
-        if (!rc) rc |= cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, counts, offsets, (int)(blocks + 1), st) != cudaSuccess;
-        if (!rc) rc |= cudaMemcpyAsync(m_host, offsets + blocks, sizeof(long long), cudaMemcpyDeviceToHost, st) != cudaSuccess;
+        PIXIE_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, counts, offsets, (int)(blocks + 1), st));
+        PIXIE_TRY(cudaMemcpyAsync(m_host, offsets + blocks, sizeof(long long), cudaMemcpyDeviceToHost, st));
     }
-    const long long* offsets = has_threshold ? counts + blocks + 1 : nullptr;
-    if (!rc) {
-        switch (K) {
-            case 1: rc = launch_decode<1>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs, opacity, cov, st); break;
-            case 4: rc = launch_decode<4>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs, opacity, cov, st); break;
-            case 9: rc = launch_decode<9>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs, opacity, cov, st); break;
-            default: rc = launch_decode<16>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs, opacity, cov, st); break;
-        }
+    cudaError_t e;
+    switch (K) {
+        case 1: e = launch_decode<1>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs, opacity, cov, st); break;
+        case 4: e = launch_decode<4>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs, opacity, cov, st); break;
+        case 9: e = launch_decode<9>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs, opacity, cov, st); break;
+        default: e = launch_decode<16>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs, opacity, cov, st); break;
     }
-    if (tmp) cudaFreeAsync(tmp, st);
-    if (counts) cudaFreeAsync(counts, st);
-    if (has_threshold) rc |= cudaStreamSynchronize(st) != cudaSuccess;
+    PIXIE_TRY(e);
+    if (has_threshold) PIXIE_TRY(cudaStreamSynchronize(st));
     else *m_host = n;
-    return rc || cudaGetLastError() != cudaSuccess;
+    return cudaSuccess;
 }
 
 }  // namespace pixie

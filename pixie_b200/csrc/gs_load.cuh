@@ -16,8 +16,8 @@ constexpr int kGsLoadMaxRowWords = 448;   // 128 staged rows of at most 448 word
 // table: n rows of `row_words` 4-byte words each (the PLY's binary vertex element, little-endian, on the device). Writes
 // the kept rows, in file order, to pos [.][3], shs [.][K][3], opacity [.], cov [.][6] (capacity n each) and their number
 // to *m_host. With has_threshold a row is kept when sigmoid(opacity) > threshold (strict; NaN is dropped), otherwise all
-// are. Host-synchronises on `st` once. Returns 2 for a bad K or row width, 1 on a CUDA error.
-int gaussian_checkpoint_decode(const void* table, long long n, int row_words, const GsColumns& cols, int K, int has_threshold,
-                               float threshold, float* pos, float* shs, float* opacity, float* cov, long long* m_host, cudaStream_t st);
+// are. K is 1, 4, 9 or 16 and 1 <= row_words <= kGsLoadMaxRowWords. Host-synchronises on `st` once when filtering.
+cudaError_t gaussian_checkpoint_decode(const void* table, long long n, int row_words, const GsColumns& cols, int K, int has_threshold,
+                                       float threshold, float* pos, float* shs, float* opacity, float* cov, long long* m_host, cudaStream_t st);
 
 }  // namespace pixie

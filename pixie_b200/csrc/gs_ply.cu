@@ -171,17 +171,16 @@ void launch(const float* pos, const float* cov, const float* shs, const float* o
 
 }  // namespace
 
-int gaussian_ply_records(const float* pos, const float* cov, const float* shs, int K, const float* opacity, int n, float* records,
-                         cudaStream_t st) {
-    if (K != 1 && K != 4 && K != 9 && K != 16) return 2;
-    if (n <= 0) return 0;
+cudaError_t gaussian_ply_records(const float* pos, const float* cov, const float* shs, int K, const float* opacity, int n, float* records,
+                                 cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
     switch (K) {
         case 1: launch<1>(pos, cov, shs, opacity, n, records, st); break;
         case 4: launch<4>(pos, cov, shs, opacity, n, records, st); break;
         case 9: launch<9>(pos, cov, shs, opacity, n, records, st); break;
         default: launch<16>(pos, cov, shs, opacity, n, records, st); break;
     }
-    return cudaGetLastError() != cudaSuccess;
+    return cudaGetLastError();
 }
 
 }  // namespace pixie

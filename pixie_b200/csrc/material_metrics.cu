@@ -20,6 +20,7 @@
 // through clip(x, lo, hi) (NaN passes), 2 * (x - lo), / span, - 1 with lo, hi, span = float32(hi - lo) each float32 and every
 // op one __f*_rn. The id channel is float(int64(id)) = trunc(id), with -0 written as +0.
 #include "material_metrics.cuh"
+#include "workspace.cuh"
 
 #include <cstdint>
 
@@ -179,21 +180,21 @@ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 
 
 }  // namespace
 
-int material_metrics(const float* mat, int c_mat, const float* mask, const float* seg, int n_classes, const float* cont, int n, long long V,
-                     const MaterialNorm& norm, int background_id, float* gt, long long* counts, double* sums, cudaStream_t st) {
-    if (n <= 0) return 0;
+cudaError_t material_metrics(const float* mat, int c_mat, const float* mask, const float* seg, int n_classes, const float* cont, int n, long long V,
+                             const MaterialNorm& norm, int background_id, float* gt, long long* counts, double* sums, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
     const bool vec = c_mat == 4 && V % 4 == 0 && aligned16(mat) && (!mask || aligned16(mask)) && aligned16(seg) && aligned16(cont) && aligned16(gt);
     const long long units = vec ? V / 4 : V;
     const int blocks = (int)(units <= 0 ? 1 : (units + kThreads - 1) / kThreads < kMaxBlocks ? (units + kThreads - 1) / kThreads : kMaxBlocks);
+    Workspace w(st);
     double* partial = nullptr;
-    if (cudaMallocAsync(&partial, (size_t)n * blocks * kAcc * sizeof(double), st) != cudaSuccess) return 1;
+    PIXIE_TRY(w.carve([&] { partial = w.take<double>((size_t)n * blocks * kAcc); }));
     const Args a{mat, mask, seg, cont, gt, partial, V, c_mat, n_classes, background_id, norm};
     const dim3 grid(blocks, n);
     if (vec) metrics_vec_kernel<<<grid, kThreads, 0, st>>>(a);
     else metrics_scalar_kernel<<<grid, kThreads, 0, st>>>(a);
     metrics_final_kernel<<<n, kThreads, 0, st>>>(partial, blocks, counts, sums);
-    cudaFreeAsync(partial, st);
-    return cudaGetLastError() != cudaSuccess;
+    return cudaGetLastError();
 }
 
 }  // namespace pixie

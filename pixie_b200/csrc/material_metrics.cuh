@@ -16,8 +16,8 @@ struct MaterialNorm {
 // null (then the mask is material id != background_id), seg [n][n_classes][V] logits, cont [n][3][V]. Writes gt [n][4][V]
 // (normalised density, E, nu, then the id truncated to an integer), counts [n][2] = (total, correct) and
 // sums [n][4] = (sum over voxels of (cont - gt)^2 * mask for the three channels, sum of mask), all on the device.
-// Stream-ordered; returns nonzero on a CUDA error.
-int material_metrics(const float* mat, int c_mat, const float* mask, const float* seg, int n_classes, const float* cont, int n, long long V,
-                     const MaterialNorm& norm, int background_id, float* gt, long long* counts, double* sums, cudaStream_t st);
+// Stream-ordered, no host sync.
+cudaError_t material_metrics(const float* mat, int c_mat, const float* mask, const float* seg, int n_classes, const float* cont, int n, long long V,
+                             const MaterialNorm& norm, int background_id, float* gt, long long* counts, double* sums, cudaStream_t st);
 
 }  // namespace pixie

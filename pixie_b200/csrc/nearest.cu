@@ -18,6 +18,7 @@
 //                memory; results are scattered back to query order.
 // The Morton codes decide only the order, never the answer: exactness rests on the pruning bound alone (see kSlack).
 #include "nearest.cuh"
+#include "workspace.cuh"
 
 #include <cub/cub.cuh>
 #include <cstdint>
@@ -235,63 +236,50 @@ query_kernel(const Tree t, const float* __restrict__ query, const unsigned* __re
     index[qi] = bi;
 }
 
-struct Workspace {
-    char* base = nullptr;
-    size_t off = 0;
-    template <class T> T* take(size_t count) {
-        T* p = reinterpret_cast<T*>(base + off);
-        off += (count * sizeof(T) + 255) & ~size_t(255);
-        return p;
-    }
-};
-
 }  // namespace
 
-int nearest_gaussian(const float* pos, int n, const float* query, int m, int* index, cudaStream_t st) {
-    if (m <= 0) return 0;
-    if (n <= 0) return cudaMemsetAsync(index, 0xff, (size_t)m * sizeof(int), st) != cudaSuccess;
+cudaError_t nearest_gaussian(const float* pos, int n, const float* query, int m, int* index, cudaStream_t st) {
+    if (m <= 0) return cudaSuccess;
+    if (n <= 0) {
+        PIXIE_TRY(cudaMemsetAsync(index, 0xff, (size_t)m * sizeof(int), st));
+        return cudaSuccess;
+    }
     const int L = (n + kLeaf - 1) / kLeaf;
     int P = 1;
     while (P < L) P <<= 1;
     size_t tb[2] = {0, 0};
-    cub::DeviceRadixSort::SortPairs(nullptr, tb[0], (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr, n,
-                                    0, 31, st);
-    cub::DeviceRadixSort::SortPairs(nullptr, tb[1], (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr, m,
-                                    0, 31, st);
+    PIXIE_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb[0], (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr,
+                                              n, 0, 31, st));
+    PIXIE_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb[1], (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr,
+                                              m, 0, 31, st));
     const size_t tmp_bytes = tb[0] > tb[1] ? tb[0] : tb[1];
     unsigned *bounds, *keys_in, *keys, *qkeys_in, *qkeys;
     int *vals_in, *order, *qvals_in, *qorder;
     float4 *sp, *lo, *hi;
     void* tmp;
-    auto carve = [&](Workspace& w) {
+    Workspace w(st);
+    PIXIE_TRY(w.carve([&] {
         bounds = w.take<unsigned>(6); tmp = w.take<char>(tmp_bytes);
         keys_in = w.take<unsigned>(n); keys = w.take<unsigned>(n); vals_in = w.take<int>(n); order = w.take<int>(n);
         sp = w.take<float4>(n); lo = w.take<float4>(2 * (size_t)P); hi = w.take<float4>(2 * (size_t)P);
         qkeys_in = w.take<unsigned>(m); qkeys = w.take<unsigned>(m); qvals_in = w.take<int>(m); qorder = w.take<int>(m);
-    };
-    Workspace sizing;
-    carve(sizing);
-    Workspace w;
-    if (cudaMallocAsync(reinterpret_cast<void**>(&w.base), sizing.off, st) != cudaSuccess) return 1;
-    carve(w);
+    }));
 
     const int B = 256;
-    cudaMemsetAsync(bounds, 0xff, 3 * sizeof(unsigned), st);         // encoded +max for the minima
-    cudaMemsetAsync(bounds + 3, 0, 3 * sizeof(unsigned), st);        // encoded -max for the maxima
+    PIXIE_TRY(cudaMemsetAsync(bounds, 0xff, 3 * sizeof(unsigned), st));         // encoded +max for the minima
+    PIXIE_TRY(cudaMemsetAsync(bounds + 3, 0, 3 * sizeof(unsigned), st));        // encoded -max for the maxima
     bounds_kernel<<<(n + B - 1) / B, B, 0, st>>>(pos, n, bounds);
     key_kernel<<<(n + B - 1) / B, B, 0, st>>>(pos, n, bounds, true, keys_in, vals_in);
-    cub::DeviceRadixSort::SortPairs(tmp, tb[0], keys_in, keys, vals_in, order, n, 0, 31, st);
+    PIXIE_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb[0], keys_in, keys, vals_in, order, n, 0, 31, st));
     gather_kernel<<<(n + B - 1) / B, B, 0, st>>>(pos, order, n, sp);
     leaf_box_kernel<<<(P + B - 1) / B, B, 0, st>>>(sp, n, P, lo, hi);
     for (int first = P / 2; first >= 1; first /= 2) level_box_kernel<<<(first + B - 1) / B, B, 0, st>>>(first, lo, hi);
     // non-finite queries get an ordinary (clamped) code here: they return -1 before using it
     key_kernel<<<(m + B - 1) / B, B, 0, st>>>(query, m, bounds, false, qkeys_in, qvals_in);
-    cub::DeviceRadixSort::SortPairs(tmp, tb[1], qkeys_in, qkeys, qvals_in, qorder, m, 0, 31, st);
+    PIXIE_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb[1], qkeys_in, qkeys, qvals_in, qorder, m, 0, 31, st));
     const Tree t{sp, keys, lo, hi, n, P};
     query_kernel<<<(m + kThreads - 1) / kThreads, kThreads, 0, st>>>(t, query, qkeys, qorder, m, index);
-    const int rc = cudaGetLastError() != cudaSuccess;
-    cudaFreeAsync(w.base, st);
-    return rc;
+    return cudaGetLastError();
 }
 
 }  // namespace pixie

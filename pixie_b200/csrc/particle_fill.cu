@@ -5,6 +5,7 @@
 //   fill_grids   : fill_dense_grids (:90-114) + internal_filling (:117-234): per-cell new counts, cub scans in C order of
 //                  cells, one host sync for the totals, then emission with counter-based random offsets.
 #include "particle_fill.cuh"
+#include "workspace.cuh"
 
 #include <cub/cub.cuh>
 #include <curand_kernel.h>
@@ -248,59 +249,49 @@ __global__ void emit_kernel(const int* __restrict__ add_d, const int* __restrict
 
 }  // namespace
 
-int fill_density(const float* pos, const float* opacity, const float* cov, int n, int grid_n, float grid_dx, int* count,
-                 float* density, cudaStream_t st) {
+cudaError_t fill_density(const float* pos, const float* opacity, const float* cov, int n, int grid_n, float grid_dx, int* count,
+                         float* density, cudaStream_t st) {
     const size_t cells = (size_t)grid_n * grid_n * grid_n;
-    cudaMemsetAsync(count, 0, cells * sizeof(int), st);
-    cudaMemsetAsync(density, 0, cells * sizeof(float), st);
+    PIXIE_TRY(cudaMemsetAsync(count, 0, cells * sizeof(int), st));
+    PIXIE_TRY(cudaMemsetAsync(density, 0, cells * sizeof(float), st));
     if (n > 0) fill_density_kernel<<<(n + 127) / 128, 128, 0, st>>>(pos, opacity, cov, n, grid_n, grid_dx, count, density);
-    return cudaGetLastError() != cudaSuccess;
+    return cudaGetLastError();
 }
 
-int fill_grids(int* count, const float* density, int grid_n, float grid_dx, const float origin[3], float density_thres,
-               float search_thres, int max_ppc, int exclude_dir, int ray_dir, unsigned long long seed, float* out, int max_samples,
-               int* n_dense_host, int* n_total_host, cudaStream_t st) {
+cudaError_t fill_grids(int* count, const float* density, int grid_n, float grid_dx, const float origin[3], float density_thres,
+                       float search_thres, int max_ppc, int exclude_dir, int ray_dir, unsigned long long seed, float* out, int max_samples,
+                       int* n_dense_host, int* n_total_host, cudaStream_t st) {
     const int cells = grid_n * grid_n * grid_n;
     const int blocks = (cells + 255) / 256;
     int *add_d = nullptr, *off_d = nullptr, *add_i = nullptr, *off_i = nullptr;
     unsigned char* flags = nullptr;
     void* tmp = nullptr;
     size_t tmp_bytes = 0;
-    int rc = 1;
-    const size_t ints = (size_t)(cells + 1) * sizeof(int);
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, add_d, off_d, cells + 1, st);
-    // stream-ordered workspaces: the only host sync is the one that brings back the totals
-    if (cudaMallocAsync(&add_d, ints, st) != cudaSuccess || cudaMallocAsync(&off_d, ints, st) != cudaSuccess ||
-        cudaMallocAsync(&add_i, ints, st) != cudaSuccess || cudaMallocAsync(&off_i, ints, st) != cudaSuccess ||
-        cudaMallocAsync(&flags, (size_t)cells, st) != cudaSuccess || cudaMallocAsync(&tmp, tmp_bytes, st) != cudaSuccess)
-        goto done;
+    PIXIE_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, add_d, off_d, cells + 1, st));
+    // stream-ordered workspace: the only host sync is the one that brings back the totals
+    Workspace w(st);
+    PIXIE_TRY(w.carve([&] {
+        add_d = w.take<int>(cells + 1); off_d = w.take<int>(cells + 1); add_i = w.take<int>(cells + 1); off_i = w.take<int>(cells + 1);
+        flags = w.take<unsigned char>(cells); tmp = w.take<char>(tmp_bytes);
+    }));
     // the extra last entry stays 0, so off[cells] is the total
-    cudaMemsetAsync(add_d + cells, 0, sizeof(int), st);
-    cudaMemsetAsync(add_i + cells, 0, sizeof(int), st);
+    PIXIE_TRY(cudaMemsetAsync(add_d + cells, 0, sizeof(int), st));
+    PIXIE_TRY(cudaMemsetAsync(add_i + cells, 0, sizeof(int), st));
     dense_count_kernel<<<blocks, 256, 0, st>>>(count, density, cells, density_thres, max_ppc, add_d);
     for (int axis = 0; axis < 3; ++axis)
         classify_kernel<<<(grid_n * grid_n + 127) / 128, 128, 0, st>>>(density, grid_n, search_thres, axis, ray_dir, flags);
     interior_count_kernel<<<blocks, 256, 0, st>>>(count, flags, cells, exclude_dir, max_ppc, add_i);
-    cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, add_d, off_d, cells + 1, st);
-    cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, add_i, off_i, cells + 1, st);
-    {
-        int n_int = 0;
-        if (cudaMemcpyAsync(n_dense_host, off_d + cells, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-            cudaMemcpyAsync(&n_int, off_i + cells, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-            cudaStreamSynchronize(st) != cudaSuccess)
-            goto done;
-        *n_total_host = *n_dense_host + n_int;
-        if (*n_total_host > max_samples) { rc = 3; goto done; }
-        if (*n_total_host > 0)
-            emit_kernel<<<blocks, 256, 0, st>>>(add_d, off_d, add_i, off_i, *n_dense_host, grid_n, grid_dx, origin[0], origin[1],
-                                                origin[2], seed, out);
-        rc = 0;
-    }
-done:
-    for (void* p : {(void*)tmp, (void*)flags, (void*)off_i, (void*)add_i, (void*)off_d, (void*)add_d})
-        if (p) cudaFreeAsync(p, st);
-    if (rc == 3) return 3;
-    return rc || cudaGetLastError() != cudaSuccess;
+    PIXIE_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, add_d, off_d, cells + 1, st));
+    PIXIE_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, add_i, off_i, cells + 1, st));
+    int n_int = 0;
+    PIXIE_TRY(cudaMemcpyAsync(n_dense_host, off_d + cells, sizeof(int), cudaMemcpyDeviceToHost, st));
+    PIXIE_TRY(cudaMemcpyAsync(&n_int, off_i + cells, sizeof(int), cudaMemcpyDeviceToHost, st));
+    PIXIE_TRY(cudaStreamSynchronize(st));
+    *n_total_host = *n_dense_host + n_int;
+    if (*n_total_host > 0 && *n_total_host <= max_samples)
+        emit_kernel<<<blocks, 256, 0, st>>>(add_d, off_d, add_i, off_i, *n_dense_host, grid_n, grid_dx, origin[0], origin[1], origin[2],
+                                            seed, out);
+    return cudaGetLastError();
 }
 
 }  // namespace pixie
