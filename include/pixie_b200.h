@@ -188,6 +188,26 @@ int pixie_fill_grids(int* count_dev, const float* density_dev, int grid_n, float
  * bounding-volume tree (not O(m n)). pos_dev [n][3], query_dev [m][3], index_dev [m] int32; n or m may be 0. Stream-ordered,
  * no host sync; repeat calls give identical results. */
 int pixie_nearest_gaussian(const float* pos_dev, int n, const float* query_dev, int m, int* index_dev, void* stream);
+/* ---- VLM part segmentation (pixie/voxel/segmentation.py). All three are stream-ordered, with no host sync.
+ * pixie_part_similarity: run_clip and the labels of clip_part_segmentation (:98-183) in one pass over the features. For the
+ * occupied voxels v (mask_dev[v] != 0, in index order; every voxel when mask_dev is NULL) of feat_dev [n_voxels][C] float16,
+ * f = feat[v] widened to fp32 and query_dev [P][C] fp32 unit rows: sims_dev [n][P] = (f . q_p) / |f| accumulated in fp32,
+ * probs_dev [n][P] = softmax over p of sims * inv_temperature (probs_dev may be NULL), labels_dev [n] int64 = the argmax of
+ * the probabilities (first index on ties, a NaN wins, as torch.argmax), scores_dev [n] = the probability at the label.
+ * n = n_occupied, the number of nonzero mask entries (n_voxels without a mask). A zero or NaN feature row gives NaN
+ * similarities, label 0 and a NaN score. 1 <= P <= 64, C >= 1; no fp32 copy of the features is made. */
+int pixie_part_similarity(const void* feat_dev, const uint8_t* mask_dev, int64_t n_voxels, int C, int n_occupied, const float* query_dev,
+                          int P, float inv_temperature, float* sims_dev, int64_t* labels_dev, float* scores_dev, float* probs_dev,
+                          void* stream);
+/* pixie_knn_label_vote: local_post_process_segmentation (:190-226). out_dev[q] = the mode of labels_dev over the k nearest
+ * points of pos_dev[q] (itself included) by the fp64 squared distance (dx*dx + dy*dy) + dz*dz of the float32 coordinates,
+ * ties at the k-th distance to the lowest index; a tie in count goes to the smallest label. pos_dev [n][3] finite,
+ * labels_dev / out_dev [n] int64, 1 <= k <= n. Exact, through the tree of pixie_nearest_gaussian; deterministic. */
+int pixie_knn_label_vote(const float* pos_dev, int n, const int64_t* labels_dev, int k, int64_t* out_dev, void* stream);
+/* pixie_nearest_vertex: the colour lookup of save_segmented_point_cloud (:283-301). index_dev[j] = the i minimising the fp64
+ * squared distance (dx*dx + dy*dy) + dz*dz between query_dev[j] (float32) and vert_dev[i] (float64), ties to the lowest i;
+ * -1 for a non-finite query or when no vertex is finite. vert_dev [n][3], query_dev [m][3], index_dev [m] int32. */
+int pixie_nearest_vertex(const double* vert_dev, int n, const float* query_dev, int m, int* index_dev, void* stream);
 /* ---- Gaussian-splatting rasteriser, forward only (gs_simulation.py:573-631 with `--render_img`: Inria's
  * diff-gaussian-rasterization at scale_modifier 1, prefiltered false, precomputed 3D covariances).
  * A renderer keeps its device buffers between frames and grows them when a frame needs more; once warm, a frame allocates

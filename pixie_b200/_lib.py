@@ -104,6 +104,10 @@ _SIGNATURES = {
     "pixie_fill_grids": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_float), C.c_float, C.c_float, C.c_int, C.c_int,
                                    C.c_int, C.c_ulonglong, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
     "pixie_nearest_gaussian": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "pixie_part_similarity": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pixie_knn_label_vote": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "pixie_nearest_vertex": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "pixie_gs_renderer_create": (C.c_int, [C.POINTER(C.c_void_p)]),
     "pixie_gs_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                   C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float, C.c_float, C.c_int, C.c_int,

@@ -11,6 +11,7 @@
 #include "gs_ply.cuh"
 #include "gs_load.cuh"
 #include "material_metrics.cuh"
+#include "part_segmentation.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -224,6 +225,32 @@ int pixie_nearest_gaussian(const float* pos, int n, const float* query, int m, i
     if ((n > 0 && m > 0 && !pos) || (m > 0 && (!query || !index))) return set_err("null argument");
     if (require_device()) return 1;
     return check("nearest_gaussian", pixie::nearest_gaussian(pos, n, query, m, index, (cudaStream_t)stream));
+}
+int pixie_nearest_vertex(const double* vert, int n, const float* query, int m, int* index, void* stream) {
+    if (n < 0 || m < 0) return set_err("nearest_vertex: negative count");
+    if ((n > 0 && m > 0 && !vert) || (m > 0 && (!query || !index))) return set_err("null argument");
+    if (require_device()) return 1;
+    return check("nearest_vertex", pixie::nearest_vertex(vert, n, query, m, index, (cudaStream_t)stream));
+}
+int pixie_knn_label_vote(const float* pos, int n, const int64_t* labels, int k, int64_t* out, void* stream) {
+    if (n < 0) return set_err("knn_label_vote: negative count");
+    if (n > 0 && (k < 1 || k > n)) return set_err("knn_label_vote: k must be in [1, n]");
+    if (n > 0 && (!pos || !labels || !out)) return set_err("null argument");
+    if (require_device()) return 1;
+    return check("knn_label_vote", pixie::knn_label_vote(pos, n, (const long long*)labels, k, (long long*)out, (cudaStream_t)stream));
+}
+// ------------------------------------------------------------------------------------- VLM part segmentation
+int pixie_part_similarity(const void* feat, const uint8_t* mask, int64_t n_voxels, int C, int n_occupied, const float* query, int P,
+                          float inv_temperature, float* sims, int64_t* labels, float* scores, float* probs, void* stream) {
+    if (n_voxels < 0 || n_occupied < 0) return set_err("part_similarity: negative count");
+    if (n_voxels > INT32_MAX) return set_err("part_similarity: more than 2^31 - 1 voxels");
+    if (C < 1) return set_err("part_similarity: C must be >= 1");
+    if (P < 1 || P > pixie::kMaxParts) return set_err("part_similarity: P must be in [1, " + std::to_string(pixie::kMaxParts) + "]");
+    if (n_occupied > n_voxels) return set_err("part_similarity: more occupied voxels than voxels");
+    if (n_occupied > 0 && (!feat || !query || !sims || !labels || !scores)) return set_err("null argument");
+    if (require_device()) return 1;
+    return check("part_similarity", pixie::part_similarity((const __half*)feat, mask, n_voxels, C, n_occupied, query, P, inv_temperature,
+                                                           sims, labels, scores, probs, (cudaStream_t)stream));
 }
 // ------------------------------------------------------------------------------------- Gaussian rasteriser
 int pixie_gs_renderer_create(pixie_gs_renderer_t* out) {
