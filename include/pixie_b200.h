@@ -5,7 +5,9 @@
  * maintainer would add (ctypes) is shown in INTEGRATION.md and shipped as pixie_b200/_lib.py.
  *
  * Conventions: plain pointers and sizes only (no torch types); every function returns 0 on success
- * and a non-zero code on failure, with a human-readable message available from pixie_last_error();
+ * and a non-zero code on failure. A failure always leaves a message for pixie_last_error() (one per host
+ * thread, replaced by the next failure); when a CUDA call failed it reads "<operation>: <CUDA's
+ * description>", and the thread's CUDA error is left clear, so the next call does not fail on it;
  * device pointers are BORROWED (the caller — torch in the Python shims — owns all tensors, as Warp
  * arrays alias torch memory in warp_utils.py:244-324); `stream` is a cudaStream_t passed as void*.
  * There is no CPU fallback: every entry point that computes requires an sm_90 (H100) device.

@@ -150,9 +150,14 @@ def load():
     return lib
 
 
+def last_error() -> PixieError:
+    """The library's message for the failure the last call on this thread reported."""
+    return PixieError(load().pixie_last_error().decode("utf-8", "replace"))
+
+
 def check(rc: int):
     if rc != 0:
-        raise PixieError(load().pixie_last_error().decode("utf-8", "replace"))
+        raise last_error()
 
 
 def require_device():

@@ -20,6 +20,7 @@
 // pixel mapping) so radii and composited sets agree with it; see DESIGN.md §7.
 #include "gs_render.cuh"
 #include "ptx.cuh"
+#include "workspace.cuh"
 
 #include <cub/cub.cuh>
 
@@ -263,12 +264,14 @@ int bit_width(uint32_t v) {
 
 }  // namespace
 
-struct GsRenderer {
-    std::string err;
+}  // namespace pixie
+
+// The C ABI's handle, pixie::GsRenderer.
+struct pixie_gs_renderer_s {
     // per Gaussian
     size_t cap_n = 0;
     float* depths = nullptr;
-    GsRecord* rec = nullptr;
+    pixie::GsRecord* rec = nullptr;
     unsigned long long* touched = nullptr;
     unsigned long long* offsets = nullptr;
     // per (Gaussian, tile) pair
@@ -284,33 +287,37 @@ struct GsRenderer {
     cudaEvent_t last = nullptr;                  // recorded after each frame's last kernel; the next frame waits for it
 };
 
+namespace pixie {
+
 namespace {
 
-int fail(GsRenderer* r, const std::string& what) {
-    const cudaError_t e = cudaGetLastError();
-    r->err = what + (e != cudaSuccess ? std::string(": ") + cudaGetErrorString(e) : std::string());
-    return 1;
-}
-
 template <typename T>
-bool grow(T*& p, size_t& cap, size_t need, size_t elem = sizeof(T)) {
-    if (need <= cap) return true;
-    if (p) cudaFree(p);
+cudaError_t grow(T*& p, size_t& cap, size_t need, size_t elem = sizeof(T)) {
+    if (need <= cap) return cudaSuccess;
+    const cudaError_t e = cudaFree(p);
     p = nullptr;
     cap = 0;
-    if (cudaMalloc(reinterpret_cast<void**>(&p), need * elem) != cudaSuccess) return false;
+    PIXIE_TRY(e);
+    PIXIE_TRY(cudaMalloc(reinterpret_cast<void**>(&p), need * elem));
     cap = need;
-    return true;
+    return cudaSuccess;
+}
+
+cudaError_t create_members(GsRenderer* r) {
+    PIXIE_TRY(cudaMallocHost(&r->total_host, sizeof(unsigned long long)));
+    for (auto& e : r->ev) PIXIE_TRY(cudaEventCreate(&e));
+    return cudaEventCreateWithFlags(&r->last, cudaEventDisableTiming);
 }
 
 }  // namespace
 
 GsRenderer* gs_renderer_create() {
     GsRenderer* r = new GsRenderer();
-    if (cudaMallocHost(&r->total_host, sizeof(unsigned long long)) != cudaSuccess) { delete r; return nullptr; }
-    for (auto& e : r->ev)
-        if (cudaEventCreate(&e) != cudaSuccess) { gs_renderer_destroy(r); return nullptr; }
-    if (cudaEventCreateWithFlags(&r->last, cudaEventDisableTiming) != cudaSuccess) { gs_renderer_destroy(r); return nullptr; }
+    if (const cudaError_t e = create_members(r)) {
+        gs_renderer_destroy(r);
+        fail("gs_renderer_create", e);
+        return nullptr;
+    }
     return r;
 }
 
@@ -325,8 +332,6 @@ void gs_renderer_destroy(GsRenderer* r) {
     if (r->last) cudaEventDestroy(r->last);
     delete r;
 }
-
-const char* gs_error(GsRenderer* r) { return r->err.c_str(); }
 
 namespace {
 
@@ -343,76 +348,78 @@ int render_frame(GsRenderer* r, const GsRenderArgs& a, int* n_rendered, float* p
     c.grid_y = (a.height + kTile - 1) / kTile;
     const int tiles = c.grid_x * c.grid_y;
     const int bits = bit_width((uint32_t)tiles);
+    // arrays that share one capacity are each re-allocated from zero
+    auto regrow = [](auto*& p, size_t want) { size_t cap = 0; return grow(p, cap, want); };
+    cudaError_t e;
 
     if (n > r->cap_n) {
-        size_t cap = 0;
         const size_t want = (size_t)n + n / 4;
-        bool ok = true;
-        cap = 0; ok = ok && grow(r->depths, cap, want);
-        cap = 0; ok = ok && grow(r->rec, cap, want);
-        cap = 0; ok = ok && grow(r->touched, cap, want);
-        cap = 0; ok = ok && grow(r->offsets, cap, want);
-        if (!ok) { r->cap_n = 0; return fail(r, "gs_render: device allocation (per Gaussian)"); }
+        e = regrow(r->depths, want);
+        if (e == cudaSuccess) e = regrow(r->rec, want);
+        if (e == cudaSuccess) e = regrow(r->touched, want);
+        if (e == cudaSuccess) e = regrow(r->offsets, want);
+        if (e != cudaSuccess) { r->cap_n = 0; return fail("gs_render: device allocation (per Gaussian)", e); }
         r->cap_n = want;
     }
-    if (!grow(r->ranges, r->cap_tiles, (size_t)tiles)) return fail(r, "gs_render: device allocation (tile ranges)");
+    if ((e = grow(r->ranges, r->cap_tiles, (size_t)tiles)) != cudaSuccess) return fail("gs_render: device allocation (tile ranges)", e);
 
     const bool timed = phase_ms != nullptr;
-    if (timed) cudaEventRecord(r->ev[0], st);
+    auto mark = [&](int k) { return timed ? cudaEventRecord(r->ev[k], st) : cudaSuccess; };
+    if ((e = mark(0)) != cudaSuccess) return fail("gs_render: phase event", e);
     if (n > 0)
         gs_preprocess_kernel<<<(n + 255) / 256, 256, 0, st>>>(a.means, a.cov, a.opacity, a.shs, a.colors, n, a.sh_coeffs, a.sh_degree, c,
                                                              a.radii, r->depths, r->rec, r->touched);
-    if (timed) cudaEventRecord(r->ev[1], st);
+    if ((e = mark(1)) != cudaSuccess) return fail("gs_render: phase event", e);
 
     unsigned long long total = 0;
     if (n > 0) {
         size_t need = 0;
-        cub::DeviceScan::InclusiveSum(nullptr, need, r->touched, r->offsets, n, st);
-        if (!grow(reinterpret_cast<char*&>(r->tmp), r->cap_tmp, need, 1)) return fail(r, "gs_render: device allocation (scan)");
-        if (cub::DeviceScan::InclusiveSum(r->tmp, need, r->touched, r->offsets, n, st) != cudaSuccess) return fail(r, "gs_render: scan");
-        if (cudaMemcpyAsync(r->total_host, r->offsets + (n - 1), sizeof(unsigned long long), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-            cudaStreamSynchronize(st) != cudaSuccess)
-            return fail(r, "gs_render: reading the pair count");
+        if ((e = cub::DeviceScan::InclusiveSum(nullptr, need, r->touched, r->offsets, n, st)) != cudaSuccess) return fail("gs_render: scan", e);
+        if ((e = grow(reinterpret_cast<char*&>(r->tmp), r->cap_tmp, need, 1)) != cudaSuccess) return fail("gs_render: device allocation (scan)", e);
+        if ((e = cub::DeviceScan::InclusiveSum(r->tmp, need, r->touched, r->offsets, n, st)) != cudaSuccess) return fail("gs_render: scan", e);
+        e = cudaMemcpyAsync(r->total_host, r->offsets + (n - 1), sizeof(unsigned long long), cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) return fail("gs_render: reading the pair count", e);
         total = *r->total_host;
     }
     if (total > 0x7fffffffull)
-        return fail(r, "gs_render: " + std::to_string(total) + " (Gaussian, tile) pairs exceed 2^31 - 1");
+        return fail("gs_render: " + std::to_string(total) + " (Gaussian, tile) pairs exceed 2^31 - 1");
     const int L = (int)total;
     if (L > 0) {
         if ((size_t)L > r->cap_pairs) {
-            size_t cap = 0;
             const size_t want = (size_t)L + L / 4;
-            bool ok = true;
-            cap = 0; ok = ok && grow(r->keys_in, cap, want);
-            cap = 0; ok = ok && grow(r->keys_out, cap, want);
-            cap = 0; ok = ok && grow(r->vals_in, cap, want);
-            cap = 0; ok = ok && grow(r->vals_out, cap, want);
-            if (!ok) { r->cap_pairs = 0; return fail(r, "gs_render: device allocation (pairs)"); }
+            e = regrow(r->keys_in, want);
+            if (e == cudaSuccess) e = regrow(r->keys_out, want);
+            if (e == cudaSuccess) e = regrow(r->vals_in, want);
+            if (e == cudaSuccess) e = regrow(r->vals_out, want);
+            if (e != cudaSuccess) { r->cap_pairs = 0; return fail("gs_render: device allocation (pairs)", e); }
             r->cap_pairs = want;
         }
         gs_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, r->rec, r->depths, a.radii, r->offsets, c.grid_x, c.grid_y, r->keys_in,
                                                        r->vals_in);
     }
-    if (timed) cudaEventRecord(r->ev[2], st);
+    if ((e = mark(2)) != cudaSuccess) return fail("gs_render: phase event", e);
     if (L > 0) {
         size_t need = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, need, r->keys_in, r->keys_out, r->vals_in, r->vals_out, L, 0, 32 + bits, st);
-        if (!grow(reinterpret_cast<char*&>(r->tmp), r->cap_tmp, need, 1)) return fail(r, "gs_render: device allocation (sort)");
-        if (cub::DeviceRadixSort::SortPairs(r->tmp, need, r->keys_in, r->keys_out, r->vals_in, r->vals_out, L, 0, 32 + bits, st) !=
+        if ((e = cub::DeviceRadixSort::SortPairs(nullptr, need, r->keys_in, r->keys_out, r->vals_in, r->vals_out, L, 0, 32 + bits, st)) != cudaSuccess)
+            return fail("gs_render: sort", e);
+        if ((e = grow(reinterpret_cast<char*&>(r->tmp), r->cap_tmp, need, 1)) != cudaSuccess) return fail("gs_render: device allocation (sort)", e);
+        if ((e = cub::DeviceRadixSort::SortPairs(r->tmp, need, r->keys_in, r->keys_out, r->vals_in, r->vals_out, L, 0, 32 + bits, st)) !=
             cudaSuccess)
-            return fail(r, "gs_render: sort");
+            return fail("gs_render: sort", e);
     }
-    if (timed) cudaEventRecord(r->ev[3], st);
-    cudaMemsetAsync(r->ranges, 0, (size_t)tiles * sizeof(uint2), st);
+    if ((e = mark(3)) != cudaSuccess) return fail("gs_render: phase event", e);
+    if ((e = cudaMemsetAsync(r->ranges, 0, (size_t)tiles * sizeof(uint2), st)) != cudaSuccess) return fail("gs_render: clearing the tile ranges", e);
     if (L > 0) gs_ranges_kernel<<<(L + 255) / 256, 256, 0, st>>>(L, r->keys_out, r->ranges);
-    if (timed) cudaEventRecord(r->ev[4], st);
+    if ((e = mark(4)) != cudaSuccess) return fail("gs_render: phase event", e);
     gs_blend_kernel<<<dim3(c.grid_x, c.grid_y), dim3(kTile, kTile), 0, st>>>(r->ranges, r->vals_out, r->rec, c.W, c.H,
                                                                           make_float3(a.bg[0], a.bg[1], a.bg[2]), a.image);
-    if (timed) cudaEventRecord(r->ev[5], st);
-    if (cudaGetLastError() != cudaSuccess) return fail(r, "gs_render: kernel launch");
+    if ((e = mark(5)) != cudaSuccess) return fail("gs_render: phase event", e);
+    if ((e = cudaGetLastError()) != cudaSuccess) return fail("gs_render: kernel launch", e);
     if (timed) {
-        if (cudaEventSynchronize(r->ev[5]) != cudaSuccess) return fail(r, "gs_render: phase timing");
-        for (int k = 0; k < 5; ++k) cudaEventElapsedTime(&phase_ms[k], r->ev[k], r->ev[k + 1]);
+        if ((e = cudaEventSynchronize(r->ev[5])) != cudaSuccess) return fail("gs_render: phase timing", e);
+        for (int k = 0; k < 5; ++k)
+            if ((e = cudaEventElapsedTime(&phase_ms[k], r->ev[k], r->ev[k + 1])) != cudaSuccess) return fail("gs_render: phase timing", e);
     }
     if (n_rendered) *n_rendered = L;
     return 0;
@@ -421,10 +428,11 @@ int render_frame(GsRenderer* r, const GsRenderArgs& a, int* n_rendered, float* p
 }  // namespace
 
 int gs_render(GsRenderer* r, const GsRenderArgs& a, int* n_rendered, float* phase_ms, cudaStream_t st) {
-    if (cudaStreamWaitEvent(st, r->last, 0) != cudaSuccess) return fail(r, "gs_render: waiting for the previous frame");
+    if (const cudaError_t e = cudaStreamWaitEvent(st, r->last, 0)) return fail("gs_render: waiting for the previous frame", e);
     const int rc = render_frame(r, a, n_rendered, phase_ms, st);
     // recorded on failure too: whatever the frame enqueued before failing still reads and writes the shared buffers
-    if (cudaEventRecord(r->last, st) != cudaSuccess && rc == 0) return fail(r, "gs_render: recording the frame's end");
+    const cudaError_t e = cudaEventRecord(r->last, st);
+    if (e != cudaSuccess && rc == 0) return fail("gs_render: recording the frame's end", e);
     return rc;
 }
 

@@ -14,6 +14,7 @@
 #include "mpm.cuh"
 #include "mpm_math.cuh"
 #include "ptx.cuh"
+#include "workspace.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -168,24 +169,26 @@ __global__ void mpm_select_cyl_kernel(const DevState s, float3 point, float3 nor
 
 }  // namespace
 
+}  // namespace pixie
+
 // ============================================================================================ host
-struct Mpm {
+// The C ABI's handle, pixie::Mpm.
+struct pixie_mpm_s {
     int n = 0, n_grid = 0;
     int n_active = 0;                  // particles [0, n_active) are live (slab mode migrates particles between ranks)
     int x_begin = 0, x_end = 0;        // grid planes this instance updates ([0, n_grid) unless slab-decomposed)
     float grid_lim = 1.f;
     void* fields[PIXIE_MPM_FIELD_COUNT] = {nullptr};
     pixie_mpm_params params{};
-    std::vector<DevBC> bcs;
+    std::vector<pixie::DevBC> bcs;
     float4* grid_mv = nullptr;
     float4* grid_v = nullptr;
-    DevBC* d_bcs = nullptr;
+    pixie::DevBC* d_bcs = nullptr;
     bool graph_valid = false;          // false: parameters / BCs changed, captured launches are stale
     // a few cached CUDA graphs keyed by (substep count, clock parity + grid parity, dt)
     static constexpr int kGraphSlots = 4;
     struct GraphSlot { cudaGraphExec_t exec = nullptr; int count = 0, parity = 0, launches = 0; double dt = 0; } graphs[kGraphSlots];
     int graph_next = 0;
-    std::string error;
 
     // ---- cell order (radix sort of base-cell keys) = physical order of the private particle copy
     int *cell_order = nullptr, *cell_keys = nullptr, *cell_keys_sorted = nullptr, *cell_idx = nullptr;
@@ -216,6 +219,8 @@ struct Mpm {
     long long launches = 0;            // kernels of this library launched for this handle (bench.py's gpu_launches)
 };
 
+namespace pixie {
+
 static constexpr int kFusedGraphSteps = 50;    // substeps per graph replay
 static constexpr int kMinGraphSteps = 4;       // shorter batches are launched directly
 static constexpr int kResortEvery = 100;       // substeps between re-sorts; CFL keeps a particle within ~a cell of its slot far longer
@@ -244,21 +249,27 @@ static DevState make_state(Mpm* m) {
     return s;
 }
 
-void mpm_destroy(Mpm* m);
-int mpm_sync(Mpm* m, cudaStream_t st);
-static void fused_launch(Mpm* m, bool do_g2p, bool do_p2g, bool write_all, float dt, cudaStream_t st);
+static cudaError_t fused_launch(Mpm* m, bool do_g2p, bool do_p2g, bool write_all, float dt, cudaStream_t st);
+
+// Zero-filled device array in `p`, unless it is already allocated: a call refused part-way allocates only the rest when
+// it is repeated.
+template <typename T>
+static cudaError_t zalloc(T*& p, size_t bytes) {
+    if (p) return cudaSuccess;
+    void* q = nullptr;
+    PIXIE_TRY(cudaMalloc(&q, bytes));
+    p = static_cast<T*>(q);
+    PIXIE_TRY(cudaMemset(q, 0, bytes));
+    return cudaSuccess;
+}
 
 // ---------------------------------------------------------------------------------- sort scratch (both paths)
-static int sort_alloc(Mpm* m) {
-    if (m->cell_order) return 0;
-    const size_t cap = (size_t)m->n;
-    if (cudaMalloc(&m->cell_order, cap * sizeof(int)) != cudaSuccess || cudaMalloc(&m->cell_keys, cap * sizeof(int)) != cudaSuccess ||
-        cudaMalloc(&m->cell_keys_sorted, cap * sizeof(int)) != cudaSuccess || cudaMalloc(&m->cell_idx, cap * sizeof(int)) != cudaSuccess) {
-        m->error = "cudaMalloc failed (cell order)"; return 1;
-    }
-    cub::DeviceRadixSort::SortPairs(nullptr, m->cub_bytes, m->cell_keys, m->cell_keys_sorted, m->cell_idx, m->cell_order, (int)cap, 0, 32, 0);
-    if (cudaMalloc(&m->cub_tmp, m->cub_bytes) != cudaSuccess) { m->error = "cudaMalloc failed (sort scratch)"; return 1; }
-    return 0;
+static cudaError_t sort_alloc(Mpm* m) {
+    const size_t bytes = (size_t)m->n * sizeof(int);
+    for (int** p : {&m->cell_order, &m->cell_keys, &m->cell_keys_sorted, &m->cell_idx}) PIXIE_TRY(zalloc(*p, bytes));
+    if (!m->cub_tmp)
+        PIXIE_TRY(cub::DeviceRadixSort::SortPairs(nullptr, m->cub_bytes, m->cell_keys, m->cell_keys_sorted, m->cell_idx, m->cell_order, m->n, 0, 32, 0));
+    return zalloc(m->cub_tmp, m->cub_bytes);
 }
 static int key_bits(const Mpm* m) {
     int bits = 1;
@@ -278,87 +289,80 @@ static FsUser fs_user(Mpm* m) {
     return u;
 }
 
-static int fused_alloc(Mpm* m) {
-    if (m->fs[0].f) return 0;
+static cudaError_t fused_alloc(Mpm* m) {
     m->cap = (m->n + 31) / 32 * 32;
     const size_t cap = (size_t)m->cap;
-    bool ok = true;
-    for (int b = 0; b < 2 && ok; ++b) {
-        Mpm::FsBuf& s = m->fs[b];
-        ok = cudaMalloc(&s.f, (size_t)FS_NFLOAT * cap * sizeof(float)) == cudaSuccess && cudaMalloc(&s.material, cap * sizeof(int)) == cudaSuccess &&
-             cudaMalloc(&s.selection, cap * sizeof(int)) == cudaSuccess && cudaMalloc(&s.perm, cap * sizeof(int)) == cudaSuccess;
-        if (ok) {
-            cudaMemset(s.f, 0, (size_t)FS_NFLOAT * cap * sizeof(float));
-            cudaMemset(s.material, 0, cap * sizeof(int)); cudaMemset(s.selection, 0, cap * sizeof(int)); cudaMemset(s.perm, 0, cap * sizeof(int));
-        }
+    for (Mpm::FsBuf& s : m->fs) {
+        PIXIE_TRY(zalloc(s.f, (size_t)FS_NFLOAT * cap * sizeof(float)));
+        PIXIE_TRY(zalloc(s.material, cap * sizeof(int)));
+        PIXIE_TRY(zalloc(s.selection, cap * sizeof(int)));
+        PIXIE_TRY(zalloc(s.perm, cap * sizeof(int)));
     }
-    if (!ok) { m->error = "cudaMalloc failed (sorted particle state)"; return 1; }
     return sort_alloc(m);
 }
 
 // node box of the particles at `x` (+ margin) into m->d_box
-static void fused_box(Mpm* m, const float* x, long long stride_comp, long long stride_part, cudaStream_t st) {
+static cudaError_t fused_box(Mpm* m, const float* x, long long stride_comp, long long stride_part, cudaStream_t st) {
     const int init[6] = {m->n_grid, m->n_grid, m->n_grid, 0, 0, 0};
-    cudaMemcpyAsync(m->d_box, init, sizeof(init), cudaMemcpyHostToDevice, st);
+    PIXIE_TRY(cudaMemcpyAsync(m->d_box, init, sizeof(init), cudaMemcpyHostToDevice, st));
     const float inv_dx = (float)((double)m->n_grid / (double)m->grid_lim);
     fs_box_kernel<<<132, 256, 0, st>>>(x, stride_comp, stride_part, m->n_active, inv_dx, m->n_grid, kBoxMargin, m->d_box, 0);
     fs_box_kernel<<<1, 32, 0, st>>>(x, stride_comp, stride_part, m->n_active, inv_dx, m->n_grid, kBoxMargin, m->d_box, 1);
     m->launches += 2;
+    return cudaSuccess;
 }
 
-static int fused_sort(Mpm* m, const float* x, long long stride_comp, long long stride_part, cudaStream_t st) {
+static cudaError_t fused_sort(Mpm* m, const float* x, long long stride_comp, long long stride_part, cudaStream_t st) {
     m->steps_since_sort = 0;
-    if (m->n_active <= 0) return 0;
+    if (m->n_active <= 0) return cudaSuccess;
     const float inv_dx = (float)((double)m->n_grid / (double)m->grid_lim);
     fs_key_kernel<<<(m->n_active + 255) / 256, 256, 0, st>>>(x, stride_comp, stride_part, m->n_active, inv_dx, m->n_grid, m->cell_keys, m->cell_idx);
     size_t bytes = m->cub_bytes;
-    if (cub::DeviceRadixSort::SortPairs(m->cub_tmp, bytes, m->cell_keys, m->cell_keys_sorted, m->cell_idx, m->cell_order, m->n_active, 0, key_bits(m), st) != cudaSuccess) {
-        m->error = "radix sort failed"; return 1;
-    }
+    PIXIE_TRY(cub::DeviceRadixSort::SortPairs(m->cub_tmp, bytes, m->cell_keys, m->cell_keys_sorted, m->cell_idx, m->cell_order, m->n_active, 0, key_bits(m), st));
     m->steps_since_sort = 0;
     m->launches += 1;          // + the radix sort passes of cub (library kernels, not counted)
-    return 0;
+    return cudaSuccess;
 }
 
 // caller's arrays -> sorted state
-static int fused_gather_from_user(Mpm* m, cudaStream_t st) {
-    if (fused_alloc(m)) return 1;
+static cudaError_t fused_gather_from_user(Mpm* m, cudaStream_t st) {
+    PIXIE_TRY(fused_alloc(m));
     const FsUser u = fs_user(m);
-    if (fused_sort(m, u.x, 1, 3, st)) return 1;
+    PIXIE_TRY(fused_sort(m, u.x, 1, 3, st));
     Mpm::FsBuf& d = m->fs[0];
     if (m->n_active > 0) fs_gather_kernel<<<(m->n_active + 255) / 256, 256, 0, st>>>(u, m->cell_order, m->n_active, m->cap, d.f, d.material, d.selection, d.perm,
                                                           m->params.update_cov_with_F ? 1 : 0);
-    fused_box(m, u.x, 1, 3, st);
+    PIXIE_TRY(fused_box(m, u.x, 1, 3, st));
     m->launches += 1;
     m->internal_valid = true;
     m->user_stale = false;
-    return cudaGetLastError() != cudaSuccess;
+    return cudaGetLastError();
 }
 
 // re-sort of the live sorted state (between two launches of the particle kernel)
-static int fused_resort(Mpm* m, cudaStream_t st) {
+static cudaError_t fused_resort(Mpm* m, cudaStream_t st) {
     Mpm::FsBuf& a = m->fs[0];
     Mpm::FsBuf& b = m->fs[1];
-    if (fused_sort(m, a.f + (size_t)FS_X * m->cap, m->cap, 1, st)) return 1;
-    if (m->n_active <= 0) return 0;
+    PIXIE_TRY(fused_sort(m, a.f + (size_t)FS_X * m->cap, m->cap, 1, st));
+    if (m->n_active <= 0) return cudaSuccess;
     fs_permute_kernel<<<(m->n_active + 255) / 256, 256, 0, st>>>(a.f, a.material, a.selection, a.perm, m->cell_order, m->n_active, m->cap, b.f, b.material,
                                                            b.selection, b.perm);
     // back into buffer 0: the captured graph and the launch arguments keep pointing at it
     const size_t cap = (size_t)m->cap;
-    cudaMemcpyAsync(a.f, b.f, (size_t)FS_NFLOAT * cap * sizeof(float), cudaMemcpyDeviceToDevice, st);
-    cudaMemcpyAsync(a.material, b.material, cap * sizeof(int), cudaMemcpyDeviceToDevice, st);
-    cudaMemcpyAsync(a.selection, b.selection, cap * sizeof(int), cudaMemcpyDeviceToDevice, st);
-    cudaMemcpyAsync(a.perm, b.perm, cap * sizeof(int), cudaMemcpyDeviceToDevice, st);
-    fused_box(m, a.f + (size_t)FS_X * m->cap, m->cap, 1, st);
+    PIXIE_TRY(cudaMemcpyAsync(a.f, b.f, (size_t)FS_NFLOAT * cap * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    PIXIE_TRY(cudaMemcpyAsync(a.material, b.material, cap * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    PIXIE_TRY(cudaMemcpyAsync(a.selection, b.selection, cap * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    PIXIE_TRY(cudaMemcpyAsync(a.perm, b.perm, cap * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    PIXIE_TRY(fused_box(m, a.f + (size_t)FS_X * m->cap, m->cap, 1, st));
     m->launches += 1;
-    return cudaGetLastError() != cudaSuccess;
+    return cudaGetLastError();
 }
 
 // sorted state -> caller's arrays (if it is ahead); afterwards the caller may mutate its arrays, so the sorted copy is
 // considered out of date.
 int mpm_sync(Mpm* m, cudaStream_t st) {
     if (m->g2p_pending && m->internal_valid) {        // slab phases: finish the last substep (gather) before anything is read
-        fused_launch(m, true, false, true, m->slab_dt, st);
+        if (const cudaError_t e = fused_launch(m, true, false, true, m->slab_dt, st)) return fail("mpm_sync", e);
         m->g2p_pending = false;
     }
     if (m->user_stale) {
@@ -366,7 +370,7 @@ int mpm_sync(Mpm* m, cudaStream_t st) {
         if (m->n_active > 0) fs_unsort_kernel<<<(m->n_active + 255) / 256, 256, 0, st>>>(fs_user(m), s.perm, m->n_active, m->cap, s.f, m->params.update_cov_with_F ? 1 : 0);
         m->user_stale = false;
         m->launches += 1;
-        if (cudaGetLastError() != cudaSuccess) { m->error = "unsort launch failed"; return 1; }
+        if (const cudaError_t e = cudaGetLastError()) return fail("mpm_sync", e);
     }
     m->internal_valid = false;
     return 0;
@@ -375,7 +379,7 @@ int mpm_sync(Mpm* m, cudaStream_t st) {
 // Launch with programmatic stream serialisation (PDL): the kernel may be scheduled while its predecessor in the stream
 // (or captured graph) is still draining; both kernels of the substep chain wait for it with griddepcontrol.wait.
 template <typename... KArgs, typename... Args>
-static void pdl_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, Args... args) {
+static cudaError_t pdl_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, Args... args) {
     static const bool pdl = !(getenv("PIXIE_MPM_PDL") && atoi(getenv("PIXIE_MPM_PDL")) == 0);
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = 0; cfg.stream = st;
@@ -383,13 +387,12 @@ static void pdl_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+    return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
 static inline size_t grid_bytes(const Mpm* m) { return (size_t)m->n_grid * m->n_grid * m->n_grid * sizeof(float4); }
 static inline float4* scatter_grid(Mpm* m) { return (m->slab && m->gpar) ? m->grid_mv_alt : m->grid_mv; }
 static inline int graph_parity(const Mpm* m) { return m->tpar | (m->gpar << 1); }
-
 static FusedState fused_state(Mpm* m) {
     FusedState t{};
     const Mpm::FsBuf& s = m->fs[0];
@@ -425,7 +428,7 @@ static FusedState fused_state(Mpm* m) {
     return t;
 }
 
-static void fused_launch(Mpm* m, bool do_g2p, bool do_p2g, bool write_all, float dt, cudaStream_t st) {
+static cudaError_t fused_launch(Mpm* m, bool do_g2p, bool do_p2g, bool write_all, float dt, cudaStream_t st) {
     FusedState t = fused_state(m);
     t.do_g2p = do_g2p; t.do_p2g = do_p2g; t.write_all = write_all;
     t.time = m->tslots + m->tpar;                 // clock of the substep whose stress / scatter runs in this launch
@@ -436,11 +439,11 @@ static void fused_launch(Mpm* m, bool do_g2p, bool do_p2g, bool write_all, float
     void (*kern)(const FusedState, const float) = mpm_fused_kernel<2, false>;
     if (hoist) kern = m->agg == 0 ? mpm_fused_kernel<0, true> : (m->agg == 1 ? mpm_fused_kernel<1, true> : (m->agg == 3 ? mpm_fused_kernel<3, true> : mpm_fused_kernel<2, true>));
     else kern = m->agg == 0 ? mpm_fused_kernel<0, false> : (m->agg == 1 ? mpm_fused_kernel<1, false> : (m->agg == 3 ? mpm_fused_kernel<3, false> : mpm_fused_kernel<2, false>));
-    pdl_launch(kern, dim3(blocks), dim3(B), st, t, dt);
     m->launches += 1;
+    return pdl_launch(kern, dim3(blocks), dim3(B), st, t, dt);
 }
 
-static void gridbox_launch(Mpm* m, bool publish_scatter, float dt, double dt_d, cudaStream_t st) {
+static cudaError_t gridbox_launch(Mpm* m, bool publish_scatter, float dt, double dt_d, cudaStream_t st) {
     GridBoxArgs g{};
     g.grid_mv = scatter_grid(m); g.grid_v = m->grid_v; g.box = m->d_box;
     g.time_in = m->tslots + m->tpar; g.time_out = m->tslots + (m->tpar ^ 1);
@@ -461,20 +464,27 @@ static void gridbox_launch(Mpm* m, bool publish_scatter, float dt, double dt_d, 
     const pixie_mpm_params& q = m->params;
     g.gx = q.gravity[0]; g.gy = q.gravity[1]; g.gz = q.gravity[2]; g.grid_v_damping_scale = q.grid_v_damping_scale;
     // enough blocks for two per SM; the kernel strides over the (usually much smaller than n_grid^3) node box
-    pdl_launch(mpm_gridbox_kernel, dim3(296), dim3(256), st, g, dt, dt_d);
+    const cudaError_t e = pdl_launch(mpm_gridbox_kernel, dim3(296), dim3(256), st, g, dt, dt_d);
     m->launches += 1;
     m->tpar ^= 1;
     if (m->slab) m->gpar ^= 1;
+    return e;
 }
 
 // `count` substeps as: scatter(0) | grid(0) | g2p(0)+scatter(1) | ... | grid(count-1) | g2p(count-1)
-static void fused_batch(Mpm* m, int count, float dt, double dt_d, cudaStream_t st) {
-    fused_launch(m, false, true, count == 1, dt, st);
+static cudaError_t fused_batch(Mpm* m, int count, float dt, double dt_d, cudaStream_t st) {
+    PIXIE_TRY(fused_launch(m, false, true, count == 1, dt, st));
     for (int i = 0; i < count; ++i) {
-        gridbox_launch(m, true, dt, dt_d, st);
-        if (i + 1 < count) fused_launch(m, true, true, i + 2 == count, dt, st);
-        else fused_launch(m, true, false, true, dt, st);
+        PIXIE_TRY(gridbox_launch(m, true, dt, dt_d, st));
+        if (i + 1 < count) PIXIE_TRY(fused_launch(m, true, true, i + 2 == count, dt, st));
+        else PIXIE_TRY(fused_launch(m, true, false, true, dt, st));
     }
+    return cudaSuccess;
+}
+
+// destroys the captured substep graphs
+static void drop_graphs(Mpm* m) {
+    for (auto& g : m->graphs) if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
 }
 
 // CUDA graph of `count` substeps starting at clock parity `m->tpar` (cached: the 50-substep batch of long rollouts and, for
@@ -485,58 +495,60 @@ static cudaGraphExec_t fused_graph(Mpm* m, int count, float dt, double dt_d) {
     Mpm::GraphSlot& slot = m->graphs[m->graph_next];
     m->graph_next = (m->graph_next + 1) % Mpm::kGraphSlots;
     if (slot.exec) { cudaGraphExecDestroy(slot.exec); slot.exec = nullptr; }
-    cudaStream_t cs;
-    cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking);
+    cudaStream_t cs = nullptr;
     cudaGraph_t g = nullptr;
     const int par0 = m->tpar, gpar0 = m->gpar, key0 = graph_parity(m);
     const long long launches0 = m->launches;
-    bool ok = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
+    bool ok = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
     if (ok) {
-        fused_batch(m, count, dt, dt_d, cs);
-        ok = cudaStreamEndCapture(cs, &g) == cudaSuccess && g;
+        const cudaError_t e = fused_batch(m, count, dt, dt_d, cs);     // the capture ends whatever it returns
+        ok = cudaStreamEndCapture(cs, &g) == cudaSuccess && g && e == cudaSuccess;
     }
     slot.launches = (int)(m->launches - launches0);
     m->tpar = par0; m->gpar = gpar0;                   // capture did not run anything
     m->launches = launches0;
     if (ok) ok = cudaGraphInstantiate(&slot.exec, g, 0) == cudaSuccess;
     if (g) cudaGraphDestroy(g);
-    cudaStreamDestroy(cs);
+    if (cs) cudaStreamDestroy(cs);
     if (!ok) { cudaGetLastError(); slot.exec = nullptr; return nullptr; }
     slot.count = count; slot.parity = key0; slot.dt = dt_d;
     return slot.exec;
 }
 
-static int mpm_step_fused(Mpm* m, int n_substeps, double dt_d, cudaStream_t st) {
+static cudaError_t mpm_step_fused(Mpm* m, int n_substeps, double dt_d, cudaStream_t st) {
     const float dt = (float)dt_d;
-    if (!m->internal_valid && fused_gather_from_user(m, st)) return 1;
+    if (m->g2p_pending && m->internal_valid) {          // phase-driven substeps came first: complete the last one
+        PIXIE_TRY(fused_launch(m, true, false, true, m->slab_dt, st));
+        m->g2p_pending = false;
+    }
+    if (!m->internal_valid) PIXIE_TRY(fused_gather_from_user(m, st));
     if (!m->graph_valid) {                              // parameters / BCs / bindings changed: captured launches are stale
-        for (auto& g : m->graphs) if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
+        drop_graphs(m);
         m->graph_valid = true;
     }
     int done = 0;
     while (done < n_substeps) {
-        if (m->steps_since_sort >= kResortEvery && fused_resort(m, st)) return 1;
+        if (m->steps_since_sort >= kResortEvery) PIXIE_TRY(fused_resort(m, st));
         int count = std::min(n_substeps - done, kFusedGraphSteps);
         count = std::min(count, std::max(1, kResortEvery - m->steps_since_sort));
         cudaGraphExec_t g = count >= kMinGraphSteps ? fused_graph(m, count, dt, dt_d) : nullptr;
         if (g) {
-            if (cudaGraphLaunch(g, st) != cudaSuccess) { m->error = "cudaGraphLaunch failed"; return 1; }
+            PIXIE_TRY(cudaGraphLaunch(g, st));
             for (auto& sl : m->graphs) if (sl.exec == g) m->launches += sl.launches;
             if (count & 1) { m->tpar ^= 1; if (m->slab) m->gpar ^= 1; }   // the replay advanced the clock `count` times
         } else {
-            fused_batch(m, count, dt, dt_d, st);
+            PIXIE_TRY(fused_batch(m, count, dt, dt_d, st));
         }
         done += count;
         m->steps_since_sort += count;
     }
     m->user_stale = true;
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { m->error = std::string("kernel launch failed: ") + cudaGetErrorString(e); return 1; }
-    return 0;
+    return cudaGetLastError();
 }
 
-Mpm* mpm_create(int n_particles, int n_grid, float grid_lim, std::string& err) {
-    if (n_particles <= 0 || n_grid <= 0) { err = "n_particles and n_grid must be positive"; return nullptr; }
+Mpm* mpm_create(int n_particles, int n_grid, float grid_lim) {
+    if (n_particles <= 0 || n_grid <= 0) { fail("n_particles and n_grid must be positive"); return nullptr; }
     auto* m = new Mpm();
     m->n = n_particles; m->n_active = n_particles; m->n_grid = n_grid; m->grid_lim = grid_lim;
     m->x_begin = 0; m->x_end = n_grid;
@@ -549,21 +561,18 @@ Mpm* mpm_create(int n_particles, int n_grid, float grid_lim, std::string& err) {
     }
     m->params.softening = 0.1f;
     const size_t nodes = (size_t)n_grid * n_grid * n_grid;
-    if (cudaMalloc(&m->xbuf, sizeof(SlabFlags) + nodes * sizeof(float4)) != cudaSuccess ||
-        cudaMalloc(&m->grid_v, nodes * sizeof(float4)) != cudaSuccess ||
-        cudaMalloc(&m->d_bcs, kMaxBC * sizeof(DevBC)) != cudaSuccess ||
-        cudaMalloc(&m->d_box, 6 * sizeof(int)) != cudaSuccess ||
-        cudaMalloc(&m->tslots, 2 * sizeof(double)) != cudaSuccess ||
-        cudaMalloc(&m->pts, (size_t)2 * kMaxBC * 3 * sizeof(float)) != cudaSuccess) {
-        err = "cudaMalloc failed (no CUDA device?)";
-        delete m;
+    cudaError_t e = zalloc(m->xbuf, sizeof(SlabFlags) + nodes * sizeof(float4));
+    if (e == cudaSuccess) e = zalloc(m->grid_v, nodes * sizeof(float4));
+    if (e == cudaSuccess) e = zalloc(m->d_bcs, kMaxBC * sizeof(DevBC));
+    if (e == cudaSuccess) e = zalloc(m->d_box, 6 * sizeof(int));
+    if (e == cudaSuccess) e = zalloc(m->tslots, 2 * sizeof(double));
+    if (e == cudaSuccess) e = zalloc(m->pts, (size_t)2 * kMaxBC * 3 * sizeof(float));
+    if (e != cudaSuccess) {
+        mpm_destroy(m);
+        fail("mpm_create", e);
         return nullptr;
     }
     m->grid_mv = reinterpret_cast<float4*>(m->xbuf + sizeof(SlabFlags));
-    cudaMemset(m->xbuf, 0, sizeof(SlabFlags) + nodes * sizeof(float4));
-    cudaMemset(m->grid_v, 0, nodes * sizeof(float4));
-    cudaMemset(m->tslots, 0, 2 * sizeof(double));
-    cudaMemset(m->pts, 0, (size_t)2 * kMaxBC * 3 * sizeof(float));
     if (const char* a = getenv("PIXIE_MPM_AGG")) m->agg = std::min(3, std::max(0, atoi(a)));
     return m;
 }
@@ -573,45 +582,53 @@ void mpm_destroy(Mpm* m) {
     cudaFree(m->cell_order); cudaFree(m->cell_keys); cudaFree(m->cell_keys_sorted); cudaFree(m->cell_idx); cudaFree(m->cub_tmp);
     for (int b = 0; b < 2; ++b) { cudaFree(m->fs[b].f); cudaFree(m->fs[b].material); cudaFree(m->fs[b].selection); cudaFree(m->fs[b].perm); }
     cudaFree(m->d_box); cudaFree(m->tslots); cudaFree(m->pts);
-    for (auto& g : m->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+    drop_graphs(m);
     cudaFree(m->xbuf);
     cudaFree(m->grid_v); cudaFree(m->d_bcs);
     delete m;
 }
 
 int mpm_bind(Mpm* m, int field, void* ptr) {
-    if (field < 0 || field >= PIXIE_MPM_FIELD_COUNT) { m->error = "bad field id"; return 1; }
+    if (field < 0 || field >= PIXIE_MPM_FIELD_COUNT) return fail("bad field id");
     if (mpm_sync(m, 0)) return 1;          // flush results into the arrays bound so far before one of them changes
     m->fields[field] = ptr;
     return 0;
 }
 int mpm_set_params(Mpm* m, const pixie_mpm_params& p) {
     if (mpm_sync(m, 0)) return 1;
+    cudaError_t e = cudaSuccess;
     if (p.n_grid != m->n_grid) {
-        // set_parameters_dict re-allocates the grids when n_grid changes (mpm_solver_warp.py:318-343)
-        if (m->slab) { m->error = "n_grid cannot change in slab mode"; return 1; }
-        cudaDeviceSynchronize();
-        cudaFree(m->xbuf);
-        cudaFree(m->grid_v);
-        m->xbuf = nullptr;
+        // set_parameters_dict re-allocates the grids when n_grid changes (mpm_solver_warp.py:318-343). The new grids are
+        // allocated before the old ones are freed, so a refused allocation leaves the handle on its previous grids.
+        if (m->slab) return fail("n_grid cannot change in slab mode");
         const size_t nodes = (size_t)p.n_grid * p.n_grid * p.n_grid;
-        if (cudaMalloc(&m->xbuf, sizeof(SlabFlags) + nodes * sizeof(float4)) != cudaSuccess ||
-            cudaMalloc(&m->grid_v, nodes * sizeof(float4)) != cudaSuccess) { m->error = "cudaMalloc failed"; return 1; }
+        uint8_t* xbuf = nullptr;
+        float4* grid_v = nullptr;
+        e = zalloc(xbuf, sizeof(SlabFlags) + nodes * sizeof(float4));
+        if (e == cudaSuccess) e = zalloc(grid_v, nodes * sizeof(float4));
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();          // queued substeps may still use the previous grids
+        if (e != cudaSuccess) {
+            cudaFree(xbuf);
+            cudaFree(grid_v);
+            return fail("mpm_set_params", e);
+        }
+        std::swap(m->xbuf, xbuf);
+        std::swap(m->grid_v, grid_v);
         m->grid_mv = reinterpret_cast<float4*>(m->xbuf + sizeof(SlabFlags));
         m->grid_mv_alt = nullptr;
-        cudaMemset(m->xbuf, 0, sizeof(SlabFlags) + nodes * sizeof(float4));
-        cudaMemset(m->grid_v, 0, nodes * sizeof(float4));
         m->n_grid = p.n_grid;
         m->x_begin = 0; m->x_end = p.n_grid;
+        e = cudaFree(xbuf);
+        if (e == cudaSuccess) e = cudaFree(grid_v);
     }
     m->grid_lim = p.grid_lim;
     m->params = p;
     m->graph_valid = false;
-    return 0;
+    return e == cudaSuccess ? 0 : fail("mpm_set_params", e);
 }
 int mpm_add_bc(Mpm* m, const pixie_mpm_bc& b) {
-    if ((int)m->bcs.size() >= kMaxBC) { m->error = "too many boundary conditions (limit " + std::to_string(kMaxBC) + ")"; return 1; }
-    if (b.kind >= PIXIE_BC_IMPULSE && !b.mask_dev) { m->error = "particle BC needs a mask"; return 1; }
+    if ((int)m->bcs.size() >= kMaxBC) return fail("too many boundary conditions (limit " + std::to_string(kMaxBC) + ")");
+    if (b.kind >= PIXIE_BC_IMPULSE && !b.mask_dev) return fail("particle BC needs a mask");
     DevBC d{};
     d.kind = b.kind;
     for (int i = 0; i < 3; ++i) {
@@ -624,15 +641,16 @@ int mpm_add_bc(Mpm* m, const pixie_mpm_bc& b) {
     d.rotation_scale = b.rotation_scale; d.translation_scale = b.translation_scale;
     d.mask = b.mask_dev;
     if (mpm_sync(m, 0)) return 1;
-    m->bcs.push_back(d);
     // append in place: the device tables also hold the *moved* cuboid positions of earlier BCs
-    const size_t k = m->bcs.size() - 1;
-    cudaMemcpy(m->d_bcs + k, &d, sizeof(DevBC), cudaMemcpyHostToDevice);
-    cudaMemcpy(m->pts + 3 * k, d.point, 3 * sizeof(float), cudaMemcpyHostToDevice);
-    cudaMemcpy(m->pts + (size_t)kMaxBC * 3 + 3 * k, d.point, 3 * sizeof(float), cudaMemcpyHostToDevice);
+    const size_t k = m->bcs.size();
+    cudaError_t e = cudaMemcpy(m->d_bcs + k, &d, sizeof(DevBC), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(m->pts + 3 * k, d.point, 3 * sizeof(float), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(m->pts + (size_t)kMaxBC * 3 + 3 * k, d.point, 3 * sizeof(float), cudaMemcpyHostToDevice);
     // a pageable host-to-device cudaMemcpy may return before its DMA lands, and the next substep may run on a stream
     // that does not wait for the legacy one
-    cudaStreamSynchronize(0);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(0);
+    if (e != cudaSuccess) return fail("mpm_add_bc", e);
+    m->bcs.push_back(d);
     m->graph_valid = false;
     return 0;
 }
@@ -640,11 +658,13 @@ int mpm_clear_bcs(Mpm* m) { m->bcs.clear(); m->graph_valid = false; return 0; }
 int mpm_set_time(Mpm* m, double t) {
     const double both[2] = {t, t};
     // synchronised like the copies of mpm_add_bc
-    return cudaMemcpy(m->tslots, both, sizeof(both), cudaMemcpyHostToDevice) != cudaSuccess || cudaStreamSynchronize(0) != cudaSuccess;
+    cudaError_t e = cudaMemcpy(m->tslots, both, sizeof(both), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(0);
+    return e == cudaSuccess ? 0 : fail("mpm_set_time", e);
 }
 int mpm_get_time(Mpm* m, double* t) {
-    const double* src = m->tslots + m->tpar;
-    return cudaMemcpy(t, src, sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess;
+    const cudaError_t e = cudaMemcpy(t, m->tslots + m->tpar, sizeof(double), cudaMemcpyDeviceToHost);
+    return e == cudaSuccess ? 0 : fail("mpm_get_time", e);
 }
 
 static int check_bound(Mpm* m) {
@@ -652,19 +672,16 @@ static int check_bound(Mpm* m) {
                                PIXIE_MPM_VOL, PIXIE_MPM_MASS, PIXIE_MPM_MU, PIXIE_MPM_LAM, PIXIE_MPM_BULK,
                                PIXIE_MPM_YIELD, PIXIE_MPM_MATERIAL, PIXIE_MPM_SELECTION};
     for (int id : need)
-        if (!m->fields[id]) { m->error = "field " + std::to_string(id) + " is not bound"; return 1; }
-    if (m->params.update_cov_with_F && !m->fields[PIXIE_MPM_COV]) { m->error = "cov not bound"; return 1; }
+        if (!m->fields[id]) return fail("field " + std::to_string(id) + " is not bound");
+    if (m->params.update_cov_with_F && !m->fields[PIXIE_MPM_COV]) return fail("cov not bound");
     return 0;
 }
 
 int mpm_step(Mpm* m, int n_substeps, double dt_d, cudaStream_t st) {
     if (check_bound(m)) return 1;
     if (n_substeps <= 0) return 0;
-    if (m->g2p_pending && m->internal_valid) {          // phase-driven substeps came first: complete the last one
-        fused_launch(m, true, false, true, m->slab_dt, st);
-        m->g2p_pending = false;
-    }
-    return mpm_step_fused(m, n_substeps, dt_d, st);
+    const cudaError_t e = mpm_step_fused(m, n_substeps, dt_d, st);
+    return e == cudaSuccess ? 0 : fail("mpm_step", e);
 }
 
 #define PIXIE_SIMPLE_LAUNCH(kernel)                                                         \
@@ -672,8 +689,7 @@ int mpm_step(Mpm* m, int n_substeps, double dt_d, cudaStream_t st) {
     const DevState s = make_state(m);                                                       \
     kernel<<<(m->n + 255) / 256, 256, 0, st>>>(s);                                          \
     const cudaError_t e = cudaGetLastError();                                               \
-    if (e != cudaSuccess) { m->error = cudaGetErrorString(e); return 1; }                   \
-    return 0;
+    return e == cudaSuccess ? 0 : fail(__func__, e);
 
 int mpm_compute_mu_lam(Mpm* m, cudaStream_t st) { PIXIE_SIMPLE_LAUNCH(mpm_mu_lam_kernel) }
 int mpm_compute_bulk(Mpm* m, cudaStream_t st) { PIXIE_SIMPLE_LAUNCH(mpm_bulk_kernel) }
@@ -684,33 +700,35 @@ int mpm_compute_R_from_F(Mpm* m, cudaStream_t st) { PIXIE_SIMPLE_LAUNCH(mpm_R_fr
 int mpm_apply_additional_params(Mpm* m, const float* boxes_host, int n_boxes, cudaStream_t st) {
     if (n_boxes <= 0) return 0;
     if (mpm_sync(m, st)) return 1;
+    Workspace ws(st);
     float* d = nullptr;
-    if (cudaMalloc(&d, (size_t)n_boxes * 10 * 4) != cudaSuccess) { m->error = "cudaMalloc failed"; return 1; }
-    cudaMemcpyAsync(d, boxes_host, (size_t)n_boxes * 10 * 4, cudaMemcpyDefault, st);    // host or device source (UVA)
-    const DevState s = make_state(m);
-    mpm_additional_params_kernel<<<(m->n + 127) / 128, 128, 0, st>>>(s, d, n_boxes);
-    cudaStreamSynchronize(st);
-    cudaFree(d);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { m->error = cudaGetErrorString(e); return 1; }
-    return 0;
+    cudaError_t e = ws.carve([&] { d = ws.take<float>((size_t)n_boxes * 10); });
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d, boxes_host, (size_t)n_boxes * 10 * 4, cudaMemcpyDefault, st);    // host or device source (UVA)
+    if (e == cudaSuccess) {
+        mpm_additional_params_kernel<<<(m->n + 127) / 128, 128, 0, st>>>(make_state(m), d, n_boxes);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    return e == cudaSuccess ? 0 : fail("mpm_apply_additional_params", e);
 }
 int mpm_select_box(Mpm* m, const float* point, const float* size, int* mask, cudaStream_t st) {
     if (mpm_sync(m, st)) return 1;
     const DevState s = make_state(m);
     mpm_select_box_kernel<<<(m->n + 255) / 256, 256, 0, st>>>(s, make_float3(point[0], point[1], point[2]),
                                                               make_float3(size[0], size[1], size[2]), mask);
-    return cudaGetLastError() != cudaSuccess;
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail("mpm_select_box", e);
 }
 int mpm_select_cylinder(Mpm* m, const float* point, const float* normal, float hh, float radius, int* mask, cudaStream_t st) {
     if (mpm_sync(m, st)) return 1;
     const DevState s = make_state(m);
     mpm_select_cyl_kernel<<<(m->n + 255) / 256, 256, 0, st>>>(s, make_float3(point[0], point[1], point[2]),
                                                               make_float3(normal[0], normal[1], normal[2]), hh, radius, mask);
-    return cudaGetLastError() != cudaSuccess;
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail("mpm_select_cylinder", e);
 }
 int mpm_set_active_count(Mpm* m, int n_active) {
-    if (n_active < 0 || n_active > m->n) { m->error = "active count exceeds the bound capacity"; return 1; }
+    if (n_active < 0 || n_active > m->n) return fail("active count exceeds the bound capacity");
     if (mpm_sync(m, 0)) return 1;          // results of the old live prefix go back first; the next step re-reads the arrays
     m->n_active = n_active;
     m->graph_valid = false;
@@ -723,8 +741,9 @@ int mpm_set_active_count(Mpm* m, int n_active) {
         for (int sd = 0; sd < 2; ++sd) {
             if (!m->peer_xbuf[sd]) continue;
             const size_t off = (size_t)m->ov_lo[sd] * plane, len = (size_t)(m->ov_hi[sd] - m->ov_lo[sd]) * plane;
-            cudaMemsetAsync(reinterpret_cast<uint8_t*>(m->grid_mv) + off, 0, len, 0);
-            cudaMemsetAsync(reinterpret_cast<uint8_t*>(m->grid_mv_alt) + off, 0, len, 0);
+            for (float4* g : {m->grid_mv, m->grid_mv_alt})
+                if (const cudaError_t e = cudaMemsetAsync(reinterpret_cast<uint8_t*>(g) + off, 0, len, 0))
+                    return fail("mpm_set_active_count", e);
         }
     }
     return 0;
@@ -738,23 +757,23 @@ int mpm_exchange_buffer(Mpm* m, void** base, size_t* bytes) {
     const size_t gb = grid_bytes(m);
     if (!m->grid_mv_alt) {
         if (mpm_sync(m, 0)) return 1;
-        cudaDeviceSynchronize();
         uint8_t* nb = nullptr;
-        if (cudaMalloc(&nb, sizeof(SlabFlags) + 2 * gb) != cudaSuccess) { m->error = "cudaMalloc failed (exchange buffer)"; return 1; }
-        cudaMemset(nb, 0, sizeof(SlabFlags) + 2 * gb);
-        cudaFree(m->xbuf);
-        m->xbuf = nb;
-        m->grid_mv = reinterpret_cast<float4*>(nb + sizeof(SlabFlags));
-        m->grid_mv_alt = reinterpret_cast<float4*>(nb + sizeof(SlabFlags) + gb);
+        cudaError_t e = cudaDeviceSynchronize();
+        if (e == cudaSuccess) e = zalloc(nb, sizeof(SlabFlags) + 2 * gb);
+        if (e != cudaSuccess) return fail("mpm_exchange_buffer", e);
+        std::swap(m->xbuf, nb);
+        m->grid_mv = reinterpret_cast<float4*>(m->xbuf + sizeof(SlabFlags));
+        m->grid_mv_alt = reinterpret_cast<float4*>(m->xbuf + sizeof(SlabFlags) + gb);
         m->graph_valid = false;
+        if ((e = cudaFree(nb)) != cudaSuccess) return fail("mpm_exchange_buffer", e);
     }
     *base = m->xbuf;
     *bytes = sizeof(SlabFlags) + 2 * gb;
     return 0;
 }
 int mpm_slab_attach(Mpm* m, int x0, int x1, int slack, const void* left_xbuf, const void* right_xbuf) {
-    if (x0 < 0 || x1 > m->n_grid || x0 >= x1 || slack < 0) { m->error = "bad slab range"; return 1; }
-    if ((left_xbuf || right_xbuf) && (x1 - x0) < 2 + 2 * slack) { m->error = "slab narrower than 2 + 2*slack planes"; return 1; }
+    if (x0 < 0 || x1 > m->n_grid || x0 >= x1 || slack < 0) return fail("bad slab range");
+    if ((left_xbuf || right_xbuf) && (x1 - x0) < 2 + 2 * slack) return fail("slab narrower than 2 + 2*slack planes");
     if (mpm_sync(m, 0)) return 1;
     const int n = m->n_grid;
     m->slab = true; m->slab_x0 = x0; m->slab_x1 = x1; m->slab_slack = slack;
@@ -766,58 +785,63 @@ int mpm_slab_attach(Mpm* m, int x0, int x1, int slack, const void* left_xbuf, co
     m->x_begin = left_xbuf ? m->ov_lo[0] : 0;
     m->x_end = right_xbuf ? m->ov_hi[1] : n;
     if (!m->grid_mv_alt) { void* b; size_t nb; if (mpm_exchange_buffer(m, &b, &nb)) return 1; }
-    cudaMemset(m->xbuf, 0, sizeof(SlabFlags) + 2 * grid_bytes(m));
+    if (const cudaError_t e = cudaMemset(m->xbuf, 0, sizeof(SlabFlags) + 2 * grid_bytes(m))) return fail("mpm_slab_attach", e);
     m->gpar = 0;
     m->graph_valid = false;
     m->g2p_pending = false;
     return 0;
 }
 // One phase of a substep (single-process drivers sequence the phases of all slabs; a multi-process rank calls mpm_step).
-int mpm_slab_phase(Mpm* m, int phase, double dt_d, cudaStream_t st) {
-    if (!m->slab) { m->error = "not in slab mode"; return 1; }
-    if (check_bound(m)) return 1;
+static cudaError_t slab_phase(Mpm* m, int phase, double dt_d, cudaStream_t st) {
     const float dt = (float)dt_d;
     if (phase == 0) {
-        if (!m->internal_valid) { if (fused_gather_from_user(m, st)) return 1; m->g2p_pending = false; }
-        else if (m->steps_since_sort >= kResortEvery && fused_resort(m, st)) return 1;
-        fused_launch(m, m->g2p_pending, true, true, dt, st);
-        pdl_launch(mpm_publish_kernel, dim3(1), dim3(32), st, reinterpret_cast<SlabFlags*>(m->xbuf));
+        if (!m->internal_valid) { PIXIE_TRY(fused_gather_from_user(m, st)); m->g2p_pending = false; }
+        else if (m->steps_since_sort >= kResortEvery) PIXIE_TRY(fused_resort(m, st));
+        PIXIE_TRY(fused_launch(m, m->g2p_pending, true, true, dt, st));
+        PIXIE_TRY(pdl_launch(mpm_publish_kernel, dim3(1), dim3(32), st, reinterpret_cast<SlabFlags*>(m->xbuf)));
         m->launches += 1;
         m->g2p_pending = false;
-    } else if (phase == 1) {
-        // nothing to launch: the overlap sums are formed inside the grid sweep (kept so that drivers written for the
-        // scatter / exchange / finish sequence need no special case)
     } else if (phase == 2) {
-        gridbox_launch(m, false, dt, dt_d, st);
+        PIXIE_TRY(gridbox_launch(m, false, dt, dt_d, st));
         m->g2p_pending = true; m->slab_dt = dt;
         ++m->steps_since_sort;
         m->user_stale = true;
-    } else { m->error = "bad phase"; return 1; }
-    return cudaGetLastError() != cudaSuccess;
+    }
+    // phase 1 launches nothing: the overlap sums are formed inside the grid sweep (kept so that drivers written for the
+    // scatter / exchange / finish sequence need no special case)
+    return cudaGetLastError();
+}
+int mpm_slab_phase(Mpm* m, int phase, double dt_d, cudaStream_t st) {
+    if (!m->slab) return fail("not in slab mode");
+    if (phase < 0 || phase > 2) return fail("bad phase");
+    if (check_bound(m)) return 1;
+    const cudaError_t e = slab_phase(m, phase, dt_d, st);
+    return e == cudaSuccess ? 0 : fail("mpm_slab_phase", e);
 }
 // Planes by which the farthest live particle's stencil base lies outside this slab's [x0, x1) (sides without a neighbour do
 // not count), max-ed into the device int `d_out` (the caller zeroes it). Reads the sorted state when it is current, so a
 // migration check costs one small kernel instead of a write-back of every field.
 int mpm_slab_excursion(Mpm* m, int* d_out, cudaStream_t st) {
-    if (!m->slab) { m->error = "not in slab mode"; return 1; }
+    if (!m->slab) return fail("not in slab mode");
     if (m->n_active <= 0) return 0;
     const float inv_dx = (float)((double)m->n_grid / (double)m->grid_lim);
     const int lo = m->peer_xbuf[0] ? m->slab_x0 : -(1 << 29);
     const int hi = m->peer_xbuf[1] ? m->slab_x1 : (1 << 29);
     const bool sorted = m->internal_valid && m->fs[0].f;
     if (sorted && m->g2p_pending) {                    // phase-driven runs: positions of the last substep first
-        fused_launch(m, true, false, true, m->slab_dt, st);
+        if (const cudaError_t e = fused_launch(m, true, false, true, m->slab_dt, st)) return fail("mpm_slab_excursion", e);
         m->g2p_pending = false;
     }
     const float* x = sorted ? m->fs[0].f + (size_t)FS_X * m->cap : reinterpret_cast<const float*>(m->fields[PIXIE_MPM_X]);
-    if (!x) { m->error = "positions not bound"; return 1; }
+    if (!x) return fail("positions not bound");
     fs_excursion_kernel<<<132, 256, 0, st>>>(x, sorted ? 1 : 3, m->n_active, inv_dx, lo, hi, d_out);
     m->launches += 1;
-    return cudaGetLastError() != cudaSuccess;
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail("mpm_slab_excursion", e);
 }
 int mpm_slab_error(Mpm* m, int* flag) {
     SlabFlags f{};
-    if (cudaMemcpy(&f, m->xbuf, sizeof(f), cudaMemcpyDeviceToHost) != cudaSuccess) return 1;
+    if (const cudaError_t e = cudaMemcpy(&f, m->xbuf, sizeof(f), cudaMemcpyDeviceToHost)) return fail("mpm_slab_error", e);
     *flag = f.error;
     return 0;
 }
@@ -828,6 +852,5 @@ int mpm_grid_ptrs(Mpm* m, float** mv4, float** v4) {
     return 0;
 }
 long long mpm_launch_count(Mpm* m) { return m->launches; }
-const std::string& mpm_error(Mpm* m) { return m->error; }
 
 }  // namespace pixie

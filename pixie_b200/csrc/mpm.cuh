@@ -1,12 +1,12 @@
-// Internal C++ interface of the MPM solver core (wrapped by the C ABI in capi.cu).
+// Internal C++ interface of the MPM solver core (wrapped by the C ABI in capi.cu). Functions that return int return 0, or 1
+// with the message of pixie_last_error() set.
 #pragma once
 #include <cuda_runtime.h>
-#include <string>
 #include "../../include/pixie_b200.h"
 
 namespace pixie {
-struct Mpm;
-Mpm* mpm_create(int n_particles, int n_grid, float grid_lim, std::string& err);
+using Mpm = pixie_mpm_s;    // the C ABI's handle is the solver object itself (mpm.cu)
+Mpm* mpm_create(int n_particles, int n_grid, float grid_lim);    // nullptr on failure
 void mpm_destroy(Mpm* m);
 int mpm_bind(Mpm* m, int field, void* ptr);
 int mpm_set_params(Mpm* m, const pixie_mpm_params& p);
@@ -32,5 +32,4 @@ int mpm_slab_attach(Mpm* m, int x0, int x1, int slack, const void* left_xbuf, co
 int mpm_slab_phase(Mpm* m, int phase, double dt, cudaStream_t st);
 int mpm_slab_error(Mpm* m, int* flag);
 int mpm_slab_excursion(Mpm* m, int* d_out, cudaStream_t st);
-const std::string& mpm_error(Mpm* m);
 }  // namespace pixie

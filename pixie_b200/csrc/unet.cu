@@ -13,6 +13,7 @@
 #include "unet.cuh"
 #include "conv3d_igemm.cuh"
 #include "unet_kernels.cuh"
+#include "workspace.cuh"
 
 #include <cmath>
 #include <cstdio>
@@ -46,9 +47,12 @@ struct DevT {          // fp32 activation [NB][sp^3][C]
 
 }  // namespace
 
-struct UNet {
+}  // namespace pixie
+
+// The C ABI's handle, pixie::UNet.
+struct pixie_unet_s {
     pixie_unet_config cfg{};
-    std::map<std::string, HostTensor> params;
+    std::map<std::string, pixie::HostTensor> params;
     bool finalized = false;
     int NBmax = 1;
 
@@ -56,8 +60,8 @@ struct UNet {
     std::vector<std::function<int(cudaStream_t)>> ops;   // bound to the batch size in `cur_nb`
     std::vector<int> op_kinds;                            // PIXIE_OP_* per op
     std::vector<double> op_flops;                         // algorithmic FLOPs per op (convs only)
-    std::vector<std::unique_ptr<ConvOp>> convs;
-    std::map<std::string, DevT> named;
+    std::vector<std::unique_ptr<pixie::ConvOp>> convs;
+    std::map<std::string, pixie::DevT> named;
     int* d_err = nullptr;              // device view of h_err
     volatile int* h_err = nullptr;     // mapped pinned host flag: a convolution that gave up waiting on its pipeline sets it
     double* d_stats = nullptr;
@@ -66,12 +70,11 @@ struct UNet {
     double flops = 0;
     int n_launch = 0;
     // I/O plumbing
-    ConvOp* first_conv = nullptr;      // consumes the user's feature grid
-    ConvOp* head_conv = nullptr;       // writes the user's output
+    pixie::ConvOp* first_conv = nullptr;      // consumes the user's feature grid
+    pixie::ConvOp* head_conv = nullptr;       // writes the user's output
     int feat_cpad = 0;
     __half* feat_staging = nullptr;    // for forward_ncdhw / forward_host
     float* out_staging = nullptr;
-    std::string error;
     // whole-forward CUDA graphs, keyed by (batch, input pointer, output pointer); a few entries so that callers that
     // alternate between buffers (double-buffered host pipeline) replay instead of re-capturing
     struct GraphEntry { cudaGraphExec_t exec = nullptr; const void* feat = nullptr; float* out = nullptr; int nb = 0; };
@@ -80,13 +83,15 @@ struct UNet {
     int graph_next = 0;
     bool use_graph = true;
 
-    ~UNet() {
+    ~pixie_unet_s() {
         for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-        for (auto& c : convs) conv_plan_destroy(c->plan);
+        for (auto& c : convs) pixie::conv_plan_destroy(c->plan);
         for (void* p : allocs) cudaFree(p);
         if (h_err) cudaFreeHost(const_cast<int*>(h_err));
     }
 };
+
+namespace pixie {
 
 namespace {
 
@@ -95,23 +100,25 @@ struct Builder {
     int NB;
     bool precise;          // split-precision: every activation tensor carries a second tensor (`lo`)
     bool f8corr;           // ... holding E5M2 correction operands (precision 2) instead of the fp16 residual (precision 1)
-    std::string err;
+    bool ok = true;        // false from the first failure on; its message is the one reported, and no convolution is planned
 
     explicit Builder(UNet& un) : u(un), NB(un.NBmax), precise(un.cfg.precision >= 1), f8corr(un.cfg.precision == 2) {}
 
-    bool fail(const std::string& m) { if (err.empty()) err = m; return false; }
+    bool fail(const std::string& m) { if (ok) pixie::fail(m); return ok = false; }
+    bool fail(const char* what, cudaError_t e) { if (ok) pixie::fail(what, e); else cudaGetLastError(); return ok = false; }
 
     template <typename T>
     T* dalloc(size_t n) {
         void* p = nullptr;
-        if (cudaMalloc(&p, n * sizeof(T)) != cudaSuccess) { fail("cudaMalloc failed"); return nullptr; }
-        cudaMemset(p, 0, n * sizeof(T));
+        if (const cudaError_t e = cudaMalloc(&p, n * sizeof(T))) { fail("unet_finalize: cudaMalloc", e); return nullptr; }
         u.allocs.push_back(p);
+        if (const cudaError_t e = cudaMemset(p, 0, n * sizeof(T))) fail("unet_finalize: cudaMemset", e);
         return reinterpret_cast<T*>(p);
     }
     float* upload(const std::vector<float>& v) {
         float* d = dalloc<float>(v.size());
-        if (d) cudaMemcpy(d, v.data(), v.size() * 4, cudaMemcpyHostToDevice);
+        if (!d) return nullptr;
+        if (const cudaError_t e = cudaMemcpy(d, v.data(), v.size() * 4, cudaMemcpyHostToDevice)) fail("unet_finalize: cudaMemcpy", e);
         return d;
     }
     const HostTensor* param(const std::string& name, size_t expect_numel) {
@@ -172,6 +179,7 @@ struct Builder {
     // epilogue when possible (no split-K), else by a moments launch right after the conv.
     ConvOp* emit_conv(const std::vector<ConvIn>& ins, int sp_out, int stride, int Cout, const float* residual,
                       float* out, bool planar, const std::vector<std::string>& bias_names, DevT* want_stats = nullptr) {
+        if (!ok) return nullptr;
         auto op = std::make_unique<ConvOp>();
         const double flops_before = u.flops;
         ConvDesc& d = op->desc;
@@ -215,7 +223,10 @@ struct Builder {
         conv_pack_weights(d, wptr, cin_real, packed);
         __half* dw = dalloc<__half>(packed.size());
         if (!dw) return nullptr;
-        cudaMemcpy(dw, packed.data(), packed.size() * 2, cudaMemcpyHostToDevice);
+        if (const cudaError_t e = cudaMemcpy(dw, packed.data(), packed.size() * 2, cudaMemcpyHostToDevice)) {
+            fail("unet_finalize: cudaMemcpy", e);
+            return nullptr;
+        }
         d.weights = dw;
         std::vector<float> bias(Cout, 0.f);
         for (const auto& bn : bias_names) {
@@ -228,7 +239,11 @@ struct Builder {
         d.out = out; d.out_ld = Cout; d.out_c0 = 0; d.out_planar = planar ? 1 : 0;
         if (want_stats) { want_stats->stats = stats_slot(Cout); d.stats = want_stats->stats; }
         char e[256] = {0};
-        if (conv_plan_create(d, u.d_err, op->plan, e, sizeof(e))) { fail(e); return nullptr; }
+        if (conv_plan_create(d, u.d_err, op->plan, e, sizeof(e))) {
+            cudaGetLastError();        // a CUDA call that failed inside the planner leaves its error set
+            fail(e);
+            return nullptr;
+        }
         ConvOp* raw = op.get();
         UNet* up = &u;
         // the plan was built for NBmax; smaller batches only shrink the tile count
@@ -339,10 +354,10 @@ struct Builder {
         {   // mapped pinned flag: the host can poll it without synchronising (checked at the start of every forward
             // and after every synchronising call), the kernels write it through the device alias
             int* h = nullptr;
-            if (cudaHostAlloc(&h, sizeof(int), cudaHostAllocMapped) != cudaSuccess) return fail("cudaHostAlloc");
+            if (const cudaError_t e = cudaHostAlloc(&h, sizeof(int), cudaHostAllocMapped)) return fail("unet_finalize: cudaHostAlloc", e);
             *h = 0;
             u.h_err = h;
-            if (cudaHostGetDevicePointer(&u.d_err, h, 0) != cudaSuccess) return fail("cudaHostGetDevicePointer");
+            if (const cudaError_t e = cudaHostGetDevicePointer(&u.d_err, h, 0)) return fail("unet_finalize: cudaHostGetDevicePointer", e);
         }
         u.stats_cap = (size_t)NB * 2 * 64 * 1024;   // doubles; far above the ~70 norms x <=512 channels
         u.d_stats = dalloc<double>(u.stats_cap);
@@ -448,19 +463,20 @@ struct Builder {
             if (!u.head_conv) return false;
         }
         if (u.stats_doubles > u.stats_cap) return fail("stats arena overflow");
-        if (!err.empty()) return false;
-        return cudaDeviceSynchronize() == cudaSuccess || fail("CUDA error during finalize");
+        if (!ok) return false;
+        const cudaError_t e = cudaDeviceSynchronize();
+        return e == cudaSuccess || fail("unet_finalize", e);
     }
 };
 
 }  // namespace
 
 // ----------------------------------------------------------------------------------------- API
-UNet* unet_create(const pixie_unet_config& cfg, std::string& err) {
-    if (cfg.n_levels < 1 || cfg.n_levels > 8) { err = "n_levels out of range"; return nullptr; }
-    if (cfg.grid_size % (1 << (cfg.n_levels - 1))) { err = "grid_size must be divisible by 2^(levels-1)"; return nullptr; }
-    if (cfg.model_channels % 64) { err = "model_channels must be a multiple of 64"; return nullptr; }
-    if (cfg.precision < 0 || cfg.precision > 2) { err = "precision must be 0 (fp16), 1 (fp16x3) or 2 (fp16 + e5m2 corrections)"; return nullptr; }
+UNet* unet_create(const pixie_unet_config& cfg) {
+    if (cfg.n_levels < 1 || cfg.n_levels > 8) { fail("n_levels out of range"); return nullptr; }
+    if (cfg.grid_size % (1 << (cfg.n_levels - 1))) { fail("grid_size must be divisible by 2^(levels-1)"); return nullptr; }
+    if (cfg.model_channels % 64) { fail("model_channels must be a multiple of 64"); return nullptr; }
+    if (cfg.precision < 0 || cfg.precision > 2) { fail("precision must be 0 (fp16), 1 (fp16x3) or 2 (fp16 + e5m2 corrections)"); return nullptr; }
     auto* u = new UNet();
     u->cfg = cfg;
     u->use_graph = getenv("PIXIE_NO_GRAPH") == nullptr;
@@ -469,7 +485,7 @@ UNet* unet_create(const pixie_unet_config& cfg, std::string& err) {
 }
 
 int unet_set_tensor(UNet* u, const char* name, const float* data, const int64_t* shape, int ndim) {
-    if (u->finalized) { u->error = "set_tensor after finalize"; return 1; }
+    if (u->finalized) return fail("set_tensor after finalize");
     HostTensor t;
     size_t n = 1;
     for (int i = 0; i < ndim; ++i) { t.shape.push_back(shape[i]); n *= (size_t)shape[i]; }
@@ -481,7 +497,7 @@ int unet_set_tensor(UNet* u, const char* name, const float* data, const int64_t*
 int unet_finalize(UNet* u) {
     if (u->finalized) return 0;
     Builder b(*u);
-    if (!b.build()) { u->error = b.err.empty() ? "finalize failed" : b.err; return 1; }
+    if (!b.build()) return 1;
     u->params.clear();
     u->finalized = true;
     u->n_launch = (int)u->ops.size() + 1;   // + stats memset
@@ -489,11 +505,9 @@ int unet_finalize(UNet* u) {
 }
 
 static int enqueue_ops(UNet* u, cudaStream_t st) {
-    cudaMemsetAsync(u->d_stats, 0, u->stats_doubles * sizeof(double), st);
-    for (auto& op : u->ops) {
-        const int rc = op(st);
-        if (rc) { u->error = "kernel launch failed, cuda error " + std::to_string(rc); return 1; }
-    }
+    if (const cudaError_t e = cudaMemsetAsync(u->d_stats, 0, u->stats_doubles * sizeof(double), st)) return fail("unet_forward: statistics clear", e);
+    for (auto& op : u->ops)
+        if (const int rc = op(st)) return fail("unet_forward: kernel launch", (cudaError_t)rc);
     return 0;
 }
 
@@ -506,23 +520,23 @@ static int run_ops(UNet* u, int batch, const void* feat, float* out, cudaStream_
             UNet::GraphEntry& slot = u->graphs[u->graph_next];
             u->graph_next = (u->graph_next + 1) % UNet::kGraphSlots;
             if (slot.exec) { cudaGraphExecDestroy(slot.exec); slot.exec = nullptr; }
-            cudaStream_t cs;                      // the caller's stream may be the legacy default stream, which cannot capture
-            cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking);
+            cudaStream_t cs = nullptr;            // the caller's stream may be the legacy default stream, which cannot capture
             cudaGraph_t g = nullptr;
-            bool ok = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
+            bool ok = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking) == cudaSuccess &&
+                      cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
             if (ok) {
-                const int rc = enqueue_ops(u, cs);
+                const int rc = enqueue_ops(u, cs);      // the capture ends whatever it returns
                 ok = (cudaStreamEndCapture(cs, &g) == cudaSuccess) && g && rc == 0;
             }
             if (ok) ok = cudaGraphInstantiate(&slot.exec, g, 0) == cudaSuccess;
             if (g) cudaGraphDestroy(g);
-            cudaStreamDestroy(cs);
+            if (cs) cudaStreamDestroy(cs);
             if (!ok) { cudaGetLastError(); slot.exec = nullptr; u->use_graph = false; }
             else { slot.nb = batch; slot.feat = feat; slot.out = out; hit = &slot; }
         }
         if (hit && hit->exec) {
-            if (cudaGraphLaunch(hit->exec, st) != cudaSuccess) { u->error = "cudaGraphLaunch failed"; return 1; }
-            return 0;
+            const cudaError_t e = cudaGraphLaunch(hit->exec, st);
+            return e == cudaSuccess ? 0 : fail("unet_forward: cudaGraphLaunch", e);
         }
     }
     return enqueue_ops(u, st);
@@ -533,88 +547,90 @@ static int check_err_flag(UNet* u) {
     const int h = u->h_err ? *u->h_err : 0;
     if (h) {
         *u->h_err = 0;
-        u->error = "conv pipeline timeout (device flag " + std::to_string(h) + "): the outputs of the affected forward are invalid";
-        return 1;
+        return fail("conv pipeline timeout (device flag " + std::to_string(h) + "): the outputs of the affected forward are invalid");
     }
     return 0;
 }
 
 int unet_forward(UNet* u, const void* feat_f16, int batch, float* out, cudaStream_t st) {
-    if (!u->finalized) { u->error = "forward before finalize"; return 1; }
+    if (!u->finalized) return fail("forward before finalize");
     if (check_err_flag(u)) return 1;          // an earlier (asynchronous) forward timed out: do not hand out more garbage
-    if (batch < 1 || batch > u->NBmax) { u->error = "batch exceeds max_batch"; return 1; }
+    if (batch < 1 || batch > u->NBmax) return fail("batch exceeds max_batch");
     // point the first convolution at the caller's grid and the head at the caller's output
     ConvOp* fc = u->first_conv;
     const __half* fp = reinterpret_cast<const __half*>(feat_f16);
     char e[256] = {0};
     if (fc->desc.srcs[0].ptr != fp) {
         fc->desc.srcs[0].ptr = fp;
-        if (conv_plan_retarget(fc->desc, fc->plan, e, sizeof(e))) { u->error = e; return 1; }
+        if (conv_plan_retarget(fc->desc, fc->plan, e, sizeof(e))) return fail(e);
     }
     u->head_conv->plan.p.out = out;
     return run_ops(u, batch, feat_f16, out, st);
 }
 
-int unet_profile(UNet* u, const void* feat_f16, int batch, float* out, cudaStream_t st, float* ms, int* kinds, double* flops, int cap) {
-    if (!u->finalized) { u->error = "profile before finalize"; return -1; }
-    const int n = (int)u->ops.size();
-    if (cap < n) { u->error = "profile: buffers too small"; return -1; }
-    if (unet_forward(u, feat_f16, batch, out, st)) return -1;      // warm + retarget
-    std::vector<cudaEvent_t> ev(n + 1);
-    for (auto& e : ev) cudaEventCreate(&e);
+// The forward's launches with an event before and after each, then their times into ms. The caller destroys the events.
+static cudaError_t time_ops(UNet* u, int batch, cudaStream_t st, std::vector<cudaEvent_t>& ev, float* ms) {
+    for (auto& e : ev) PIXIE_TRY(cudaEventCreate(&e));
     u->cur_nb = batch;
-    cudaMemsetAsync(u->d_stats, 0, u->stats_doubles * sizeof(double), st);
-    cudaEventRecord(ev[0], st);
-    for (int i = 0; i < n; ++i) {
-        if (u->ops[i](st)) { u->error = "kernel launch failed"; return -1; }
-        cudaEventRecord(ev[i + 1], st);
+    PIXIE_TRY(cudaMemsetAsync(u->d_stats, 0, u->stats_doubles * sizeof(double), st));
+    PIXIE_TRY(cudaEventRecord(ev[0], st));
+    for (size_t i = 0; i < u->ops.size(); ++i) {
+        PIXIE_TRY((cudaError_t)u->ops[i](st));
+        PIXIE_TRY(cudaEventRecord(ev[i + 1], st));
     }
-    cudaStreamSynchronize(st);
+    PIXIE_TRY(cudaStreamSynchronize(st));
+    for (size_t i = 0; i < u->ops.size(); ++i) PIXIE_TRY(cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]));
+    return cudaSuccess;
+}
+
+int unet_profile(UNet* u, const void* feat_f16, int batch, float* out, cudaStream_t st, float* ms, int* kinds, double* flops, int cap) {
+    if (!u->finalized) { fail("profile before finalize"); return -1; }
+    const int n = (int)u->ops.size();
+    if (cap < n) { fail("profile: buffers too small"); return -1; }
+    if (unet_forward(u, feat_f16, batch, out, st)) return -1;      // warm + retarget
+    std::vector<cudaEvent_t> ev(n + 1, nullptr);
+    const cudaError_t e = time_ops(u, batch, st, ev, ms);
+    for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x);
+    if (e != cudaSuccess) { fail("unet_profile", e); return -1; }
     for (int i = 0; i < n; ++i) {
-        cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
         kinds[i] = u->op_kinds[i];
         flops[i] = u->op_flops[i];
     }
-    for (auto& e : ev) cudaEventDestroy(e);
     return n;
 }
 
 int unet_forward_ncdhw(UNet* u, const float* feat_f32, int batch, float* out, cudaStream_t st) {
-    if (!u->finalized) { u->error = "forward before finalize"; return 1; }
-    if (batch < 1 || batch > u->NBmax) { u->error = "batch exceeds max_batch"; return 1; }
+    if (!u->finalized) return fail("forward before finalize");
+    if (batch < 1 || batch > u->NBmax) return fail("batch exceeds max_batch");
     const long long V = (long long)u->cfg.grid_size * u->cfg.grid_size * u->cfg.grid_size;
-    if (launch_ncdhw_to_ndhwc_f16(feat_f32, u->feat_staging, batch, u->cfg.feature_channels, u->feat_cpad, V, st)) {
-        u->error = "layout conversion launch failed";
-        return 1;
-    }
+    if (const int rc = launch_ncdhw_to_ndhwc_f16(feat_f32, u->feat_staging, batch, u->cfg.feature_channels, u->feat_cpad, V, st))
+        return fail("unet_forward_ncdhw: layout conversion", (cudaError_t)rc);
     return unet_forward(u, u->feat_staging, batch, out, st);
 }
 
 int unet_forward_host(UNet* u, const void* feat_host, int batch, float* out_host, cudaStream_t st) {
-    if (!u->finalized) { u->error = "forward before finalize"; return 1; }
-    if (batch < 1 || batch > u->NBmax) { u->error = "batch exceeds max_batch"; return 1; }
-    if (u->feat_cpad != u->cfg.feature_channels) { u->error = "forward_host needs feature_channels % 64 == 0"; return 1; }
+    if (!u->finalized) return fail("forward before finalize");
+    if (batch < 1 || batch > u->NBmax) return fail("batch exceeds max_batch");
+    if (u->feat_cpad != u->cfg.feature_channels) return fail("forward_host needs feature_channels % 64 == 0");
     const size_t V = (size_t)u->cfg.grid_size * u->cfg.grid_size * u->cfg.grid_size;
-    if (cudaMemcpyAsync(u->feat_staging, feat_host, (size_t)batch * V * u->feat_cpad * 2, cudaMemcpyHostToDevice, st) != cudaSuccess) {
-        u->error = "H2D copy failed"; return 1;
-    }
+    if (const cudaError_t e = cudaMemcpyAsync(u->feat_staging, feat_host, (size_t)batch * V * u->feat_cpad * 2, cudaMemcpyHostToDevice, st))
+        return fail("unet_forward_host: host-to-device copy", e);
     if (unet_forward(u, u->feat_staging, batch, u->out_staging, st)) return 1;
-    if (cudaMemcpyAsync(out_host, u->out_staging, (size_t)batch * u->cfg.out_channels * V * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) {
-        u->error = "D2H copy failed"; return 1;
-    }
-    if (cudaStreamSynchronize(st) != cudaSuccess) { u->error = "stream sync failed"; return 1; }
+    if (const cudaError_t e = cudaMemcpyAsync(out_host, u->out_staging, (size_t)batch * u->cfg.out_channels * V * 4, cudaMemcpyDeviceToHost, st))
+        return fail("unet_forward_host: device-to-host copy", e);
+    if (const cudaError_t e = cudaStreamSynchronize(st)) return fail("unet_forward_host", e);
     return check_err_flag(u);
 }
 
 int64_t unet_debug_fetch(UNet* u, const char* name, float* host_out, int64_t capacity) {
     auto it = u->named.find(name);
-    if (it == u->named.end()) { u->error = std::string("no such activation: ") + name; return -1; }
+    if (it == u->named.end()) { fail(std::string("no such activation: ") + name); return -1; }
     const DevT& t = it->second;
     const int64_t n = (int64_t)u->cur_nb * t.sp * t.sp * t.sp * t.C;
-    if (n > capacity) { u->error = "debug_fetch: buffer too small"; return -2; }
-    if (cudaDeviceSynchronize() != cudaSuccess) { u->error = "sync failed"; return -3; }
+    if (n > capacity) { fail("debug_fetch: buffer too small"); return -2; }
+    if (const cudaError_t e = cudaDeviceSynchronize()) { fail("unet_debug_fetch", e); return -3; }
     if (check_err_flag(u)) return -4;
-    cudaMemcpy(host_out, t.p, (size_t)n * 4, cudaMemcpyDeviceToHost);
+    if (const cudaError_t e = cudaMemcpy(host_out, t.p, (size_t)n * 4, cudaMemcpyDeviceToHost)) { fail("unet_debug_fetch", e); return -3; }
     return n;
 }
 
@@ -625,7 +641,6 @@ std::string unet_debug_names(UNet* u) {
     return s;
 }
 
-const std::string& unet_error(UNet* u) { return u->error; }
 int unet_launch_count(UNet* u) {
     int n = 1;
     for (auto& c : u->convs) n += c->plan.needs_zero ? 1 : 0;
@@ -633,7 +648,7 @@ int unet_launch_count(UNet* u) {
 }
 double unet_flops(UNet* u) { return u->flops; }
 int unet_check(UNet* u) {
-    if (cudaDeviceSynchronize() != cudaSuccess) { u->error = "CUDA error"; return 1; }
+    if (const cudaError_t e = cudaDeviceSynchronize()) return fail("unet_check", e);
     return check_err_flag(u);
 }
 void unet_destroy(UNet* u) { delete u; }

@@ -1,8 +1,9 @@
-// Scratch memory and error returns of the stateless device operations behind the C ABI (those that take no handle): each
-// returns the first failing cudaError_t and leaves the thread's last error clear.
+// Error reporting of the library, and the scratch memory of the stateless device operations behind the C ABI (those that
+// take no handle): each of those returns the first failing cudaError_t and leaves the thread's last error clear.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstddef>
+#include <string>
 
 // Returns the status of `expr` from the enclosing operation when it is an error. The thread's last error is cleared first:
 // the operations check it for launch errors, so a stale one would make the next, valid call fail.
@@ -10,6 +11,14 @@
     do { const cudaError_t pixie_e_ = (expr); if (pixie_e_ != cudaSuccess) { cudaGetLastError(); return pixie_e_; } } while (0)
 
 namespace pixie {
+
+// The message pixie_last_error() returns, one per host thread, is the library's only error state (capi.cu). Both setters
+// return 1, the C ABI's failure code.
+// Refused input or state, e.g. "forward before finalize".
+int fail(const std::string& message);
+// A failed CUDA call: "<what>: <CUDA's description of e>". Also clears the thread's last error, so that the failure is not
+// blamed on the next, valid call.
+int fail(const std::string& what, cudaError_t e);
 
 // One cudaMallocAsync on the operation's stream, handed out as 256-byte aligned typed arrays and freed on that stream
 // when the workspace goes out of scope, so every return frees it.

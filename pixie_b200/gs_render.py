@@ -237,7 +237,7 @@ _RENDERERS_LOCK = threading.Lock()
 
 class _Renderer:
     """One device's renderer handle; its buffers grow to the largest frame seen and are reused. Its host-side state
-    (capacities, the pinned pair-count word, the error string) is guarded by `lock`."""
+    (capacities, the pinned pair-count word) is guarded by `lock`."""
 
     def __init__(self, device: torch.device):
         lib = _lib.require_device()

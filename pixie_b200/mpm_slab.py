@@ -62,15 +62,11 @@ class FusedSlabBackend:
         if solver._masks:
             raise ValueError("slab-decomposed runs do not migrate per-particle BC masks (impulses, velocity modifiers)")
         base, nbytes = C.c_void_p(), C.c_size_t()
-        self._check(self.lib.pixie_mpm_exchange_buffer(solver._handle, C.byref(base), C.byref(nbytes)))
+        _lib.check(self.lib.pixie_mpm_exchange_buffer(solver._handle, C.byref(base), C.byref(nbytes)))
         self.xbuf, self.xbuf_bytes = base.value, nbytes.value
         self._opened = []
         self._active = -1
         self.set_active(n_active)
-
-    def _check(self, rc: int):
-        if rc != 0:
-            raise _lib.PixieError(self.lib.pixie_last_error().decode())
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
@@ -80,20 +76,20 @@ class FusedSlabBackend:
         """64-byte cudaIpc handle of the exchange buffer, for a neighbour in another process."""
         buf = C.create_string_buffer(64)
         with torch.cuda.device(self.device):
-            self._check(self.lib.pixie_ipc_export(C.c_void_p(self.xbuf), buf))
+            _lib.check(self.lib.pixie_ipc_export(C.c_void_p(self.xbuf), buf))
         return buf.raw
 
     def open_handle(self, handle: bytes) -> int:
         p = C.c_void_p()
         with torch.cuda.device(self.device):
-            self._check(self.lib.pixie_ipc_open(C.create_string_buffer(handle, 64), C.byref(p)))
+            _lib.check(self.lib.pixie_ipc_open(C.create_string_buffer(handle, 64), C.byref(p)))
         self._opened.append(p.value)
         return p.value
 
     def attach(self, x0: int, x1: int, slack: int, left: Optional[int], right: Optional[int]):
         """Neighbours' exchange buffers as device pointers valid in this process (None at the domain ends)."""
         with torch.cuda.device(self.device):
-            self._check(self.lib.pixie_mpm_slab_attach(self.solver._handle, int(x0), int(x1), int(slack),
+            _lib.check(self.lib.pixie_mpm_slab_attach(self.solver._handle, int(x0), int(x1), int(slack),
                                                        C.c_void_p(left) if left else None, C.c_void_p(right) if right else None))
 
     def close(self):
@@ -104,7 +100,7 @@ class FusedSlabBackend:
     # -- substep phases (each only enqueues kernels)
     def _phase(self, ph: int, dt: float):
         with torch.cuda.device(self.device):
-            self._check(self.lib.pixie_mpm_slab_phase(self.solver._handle, ph, float(dt), self._stream()))
+            _lib.check(self.lib.pixie_mpm_slab_phase(self.solver._handle, ph, float(dt), self._stream()))
 
     def scatter(self, dt: float):
         self._phase(0, dt)
@@ -123,7 +119,7 @@ class FusedSlabBackend:
         flag = C.c_int(0)
         with torch.cuda.device(self.device):
             torch.cuda.current_stream(self.device).synchronize()
-            self._check(self.lib.pixie_mpm_slab_error(self.solver._handle, C.byref(flag)))
+            _lib.check(self.lib.pixie_mpm_slab_error(self.solver._handle, C.byref(flag)))
         return flag.value
 
     def excursion(self) -> torch.Tensor:
@@ -131,7 +127,7 @@ class FusedSlabBackend:
         over the sorted positions; no write-back of the particle fields, no host sync)."""
         out = torch.zeros(1, dtype=torch.int32, device=self.device)
         with torch.cuda.device(self.device):
-            self._check(self.lib.pixie_mpm_slab_excursion(self.solver._handle, C.c_void_p(out.data_ptr()), self._stream()))
+            _lib.check(self.lib.pixie_mpm_slab_excursion(self.solver._handle, C.c_void_p(out.data_ptr()), self._stream()))
         return out
 
     # -- particles
@@ -145,7 +141,7 @@ class FusedSlabBackend:
         if n > self.capacity:
             raise RuntimeError(f"slab holds {n} particles but was created with capacity {self.capacity}")
         if n != self._active or force:
-            self._check(self.lib.pixie_mpm_set_active_count(self.solver._handle, int(n)))
+            _lib.check(self.lib.pixie_mpm_set_active_count(self.solver._handle, int(n)))
             self._active = int(n)
 
     def get(self, name: str) -> torch.Tensor:

@@ -289,7 +289,7 @@ class _B200UNet:
             k = lib.pixie_unet_profile(self._handle, C.c_void_p(feat_ndhwc.data_ptr()), n, C.c_void_p(out.data_ptr()),
                                        C.c_void_p(st), ms, kinds, fl, cap)
         if k < 0:
-            raise _lib.PixieError(lib.pixie_last_error().decode())
+            raise _lib.last_error()
         names = {0: "conv", 1: "moments", 2: "norm", 3: "upsample", 4: "attention"}
         return [(names[kinds[i]], ms[i], fl[i]) for i in range(k)]
 
@@ -298,7 +298,7 @@ class _B200UNet:
         buf = torch.empty(batch * sp ** 3 * channels, dtype=torch.float32)
         n = _lib.load().pixie_unet_debug_fetch(self._handle, name.encode(), C.c_void_p(buf.data_ptr()), buf.numel())
         if n < 0:
-            raise _lib.PixieError(_lib.load().pixie_last_error().decode())
+            raise _lib.last_error()
         return buf[:n].view(batch, sp, sp, sp, channels).permute(0, 4, 1, 2, 3).contiguous()
 
     def debug_names(self) -> Dict[str, Tuple[int, int]]:
@@ -307,7 +307,7 @@ class _B200UNet:
         lib = _lib.load()
         n = lib.pixie_unet_debug_names(self._handle, None, 0)
         if n < 0:
-            raise _lib.PixieError(lib.pixie_last_error().decode())
+            raise _lib.last_error()
         buf = C.create_string_buffer(n + 1)
         lib.pixie_unet_debug_names(self._handle, buf, n + 1)
         names = {}
