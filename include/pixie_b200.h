@@ -208,6 +208,7 @@ int pixie_part_similarity(const void* feat_dev, const uint8_t* mask_dev, int64_t
 int pixie_knn_label_vote(const float* pos_dev, int n, const int64_t* labels_dev, int k, int64_t* out_dev, void* stream);
 /* pixie_nearest_vertex: the colour lookup of save_segmented_point_cloud (:283-301). index_dev[j] = the i minimising the fp64
  * squared distance (dx*dx + dy*dy) + dz*dz between query_dev[j] (float32) and vert_dev[i] (float64), ties to the lowest i;
+ * a vertex with a NaN or Inf coordinate is never chosen, a finite one is even where d2 overflows to Inf;
  * -1 for a non-finite query or when no vertex is finite. vert_dev [n][3], query_dev [m][3], index_dev [m] int32. */
 int pixie_nearest_vertex(const double* vert_dev, int n, const float* query_dev, int m, int* index_dev, void* stream);
 /* ---- Gaussian-splatting rasteriser, forward only (gs_simulation.py:573-631 with `--render_img`: Inria's

@@ -7,7 +7,9 @@
                     scipy's mode (its tie choice at the k-th distance is scikit-learn's).
   vote_exact        the same vote with the k nearest chosen by (fp64 squared distance, index), brute force.
   kth_distance_gap  per point, whether the k-th and (k+1)-th fp64 distances differ (there the two votes agree).
-  nearest_exact     the nearest float64 vertex of float32 queries by fp64 squared distance, ties to the lowest index.
+  knn_table         the K nearest of every point with their d2, one brute-force pass; vote_of and gap_of give the vote and
+                    the gap for every k <= K (K - 1 for the gap) from it.
+  nearest_exact     the nearest finite float64 vertex of float32 queries by fp64 squared distance, ties to the lowest index.
   save_files        save_segmented_point_cloud (:231-471) in numpy, with scipy's cKDTree for the colours.
 """
 from __future__ import annotations
@@ -58,38 +60,58 @@ def _d2(q: np.ndarray, p: np.ndarray) -> np.ndarray:
     return (d[0] * d[0] + d[1] * d[1]) + d[2] * d[2]
 
 
-def knn_exact(coords: np.ndarray, k: int, chunk: int = 512) -> np.ndarray:
-    """(N, k) indices of the k nearest points by (fp64 squared distance, index)."""
+def knn_table(coords: np.ndarray, kmax: int, chunk: int = 512):
+    """((N, K) indices, (N, K) fp64 squared distances) of the K = min(kmax, N) nearest points of every point by (fp64 squared
+    distance, index). The k nearest for any k <= K are the first k columns, so one table serves many k."""
     c = np.asarray(coords, np.float32)
-    out = np.empty((len(c), k), np.int64)
+    K = min(kmax, len(c))
+    idx, dist = np.empty((len(c), K), np.int64), np.empty((len(c), K), np.float64)
     for s in range(0, len(c), chunk):
         d2 = _d2(c[s:s + chunk], c)
-        out[s:s + chunk] = np.argsort(d2, axis=1, kind="stable")[:, :k]
-    return out
+        o = np.argsort(d2, axis=1, kind="stable")[:, :K]
+        idx[s:s + chunk], dist[s:s + chunk] = o, np.take_along_axis(d2, o, axis=1)
+    return idx, dist
+
+
+def knn_exact(coords: np.ndarray, k: int, chunk: int = 512) -> np.ndarray:
+    """(N, k) indices of the k nearest points by (fp64 squared distance, index)."""
+    return knn_table(coords, k, chunk)[0]
+
+
+def vote_of(labels: np.ndarray, idx: np.ndarray) -> np.ndarray:
+    """The vote over the (N, k) neighbour indices idx: per row the most frequent label, the smallest on a count tie."""
+    return _mode(np.asarray(labels, np.int64)[idx])
 
 
 def vote_exact(coords: np.ndarray, labels: np.ndarray, k: int = 200) -> np.ndarray:
-    return _mode(np.asarray(labels, np.int64)[knn_exact(coords, k)])
+    return vote_of(labels, knn_exact(coords, k))
+
+
+def gap_of(dist: np.ndarray, k: int) -> np.ndarray:
+    """kth_distance_gap from knn_table's distances with at least k + 1 columns (True everywhere when k = N)."""
+    return np.ones(len(dist), bool) if k >= len(dist) else dist[:, k - 1] != dist[:, k]
 
 
 def kth_distance_gap(coords: np.ndarray, k: int, chunk: int = 512) -> np.ndarray:
     """Per point, True where the k-th and (k+1)-th smallest fp64 squared distances differ (True when k = N)."""
-    c = np.asarray(coords, np.float32)
-    out = np.ones(len(c), bool)
-    if k >= len(c):
-        return out
-    for s in range(0, len(c), chunk):
-        d2 = np.sort(_d2(c[s:s + chunk], c), axis=1)
-        out[s:s + chunk] = d2[:, k - 1] != d2[:, k]
-    return out
+    return gap_of(knn_table(coords, k + 1, chunk)[1], k)
 
 
 def nearest_exact(vertices: np.ndarray, queries: np.ndarray, chunk: int = 512) -> np.ndarray:
-    v = np.asarray(vertices, np.float64)
-    q = np.asarray(queries, np.float32)
-    out = np.empty(len(q), np.int64)
+    """Vertices with a NaN or Inf coordinate are never chosen; among the finite ones a d2 that overflows to Inf still
+    counts (all at Inf: the lowest finite index). -1 for a non-finite query or without finite vertices."""
+    v = np.asarray(vertices, np.float64).reshape(-1, 3)
+    q = np.asarray(queries, np.float32).reshape(-1, 3)
+    out = np.full(len(q), -1, np.int64)
+    ok = np.isfinite(v).all(1)
+    if not ok.any():
+        return out
+    fin = np.flatnonzero(ok)
     for s in range(0, len(q), chunk):
-        out[s:s + chunk] = np.argmin(_d2(q[s:s + chunk], v), axis=1)      # argmin: the first of equal minima
+        with np.errstate(over="ignore", invalid="ignore"):
+            d2 = _d2(q[s:s + chunk], v[ok])
+        out[s:s + chunk] = fin[np.argmin(d2, axis=1)]           # argmin: the first of equal minima, Inf included
+    out[~np.isfinite(q).all(1)] = -1
     return out
 
 

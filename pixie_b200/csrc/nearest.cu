@@ -221,21 +221,28 @@ __device__ __forceinline__ double d2_f64(double qx, double qy, double qz, double
     return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
 }
 
-// F64 = false: the float32 distance d of nearest_gaussian, initial best 1e10. F64 = true: the fp64 squared distance to the
-// point's fp64 coordinates, initial best +Inf (so -1 only without finite points).
+// Scans the sorted points of a leaf below n_scan. F64 = false: the float32 distance d of nearest_gaussian, initial best
+// 1e10, which a d of exactly 1e10 does not beat. F64 = true: the fp64 squared distance to the point's fp64 coordinates,
+// initial best +Inf, and n_scan the number of finite points (the non-finite ones sort after them): a finite point whose d2
+// overflows to +Inf ties the initial best and takes it (unsigned bi: -1 loses every tie), so the result is -1 only
+// without finite points.
 template <bool F64> struct Best { using D = float; };
 template <> struct Best<true> { using D = double; };
 
 template <bool F64>
-__device__ __forceinline__ void scan_leaf(const Tree& t, int leaf, float qx, float qy, float qz, typename Best<F64>::D& bd, int& bi) {
-    const int e = min(t.n, (leaf + 1) * kLeaf);
+__device__ __forceinline__ void scan_leaf(const Tree& t, int leaf, int n_scan, float qx, float qy, float qz, typename Best<F64>::D& bd,
+                                          int& bi) {
+    const int e = min(n_scan, (leaf + 1) * kLeaf);
     for (int j = leaf * kLeaf; j < e; ++j) {
         const float4 p = t.sp[j];
-        typename Best<F64>::D d;
-        if constexpr (F64) d = d2_f64(qx, qy, qz, t.sd[3 * (size_t)j], t.sd[3 * (size_t)j + 1], t.sd[3 * (size_t)j + 2]);
-        else d = dist_f32(qx, qy, qz, p.x, p.y, p.z);
         const int i = __float_as_int(p.w);
-        if (d < bd || (d == bd && i < bi)) { bd = d; bi = i; }       // bi = -1 only while bd is the initial value: never tied
+        if constexpr (F64) {
+            const double d = d2_f64(qx, qy, qz, t.sd[3 * (size_t)j], t.sd[3 * (size_t)j + 1], t.sd[3 * (size_t)j + 2]);
+            if (d < bd || (d == bd && (unsigned)i < (unsigned)bi)) { bd = d; bi = i; }
+        } else {
+            const float d = dist_f32(qx, qy, qz, p.x, p.y, p.z);
+            if (d < bd || (d == bd && i < bi)) { bd = d; bi = i; }   // bi = -1 only while bd is 1e10: never tied
+        }
     }
 }
 
@@ -259,9 +266,11 @@ query_kernel(const Tree t, const float* __restrict__ query, const unsigned* __re
     if (!finite3(qx, qy, qz)) { index[qi] = -1; return; }      // every d is NaN or Inf
     typename Best<F64>::D bd = F64 ? (typename Best<F64>::D)INFINITY : (typename Best<F64>::D)kNone;
     int bi = -1;
+    // fp64 points with a NaN or Inf coordinate (code kNonFinite, sorted last) are never scanned
+    const int n_scan = F64 ? lower_bound(t.keys, t.n, kNonFinite) : t.n;
     // seed: the leaf at the query's Morton position
     const int seed = min(lower_bound(t.keys, t.n, qkeys[s]), t.n - 1) / kLeaf;
-    scan_leaf<F64>(t, seed, qx, qy, qz, bd, bi);
+    scan_leaf<F64>(t, seed, n_scan, qx, qy, qz, bd, bi);
     double thr2 = prune_above(bd);
     const double dqx = qx, dqy = qy, dqz = qz;
     const int tid = threadIdx.x;
@@ -276,7 +285,7 @@ query_kernel(const Tree t, const float* __restrict__ query, const unsigned* __re
         if (v >= t.P) {
             const int leaf = v - t.P;
             if (leaf != seed) {
-                scan_leaf<F64>(t, leaf, qx, qy, qz, bd, bi);
+                scan_leaf<F64>(t, leaf, n_scan, qx, qy, qz, bd, bi);
                 thr2 = prune_above(bd);
             }
             continue;

@@ -61,10 +61,17 @@ def normalize_queries(query_embs, device) -> torch.Tensor:
     return q / q.norm(dim=-1, keepdim=True)
 
 
+def mask_flags(mask: torch.Tensor, device) -> torch.Tensor:
+    """The mask as contiguous flat uint8 0 / 1 on `device`, selecting the rows `mask.bool()` selects: any non-zero entry (0.5,
+    -1, NaN) is occupied. A direct uint8 cast would truncate 0.5 to 0 and leave NaN undefined."""
+    return mask.to(device).reshape(-1).bool().to(torch.uint8).contiguous()
+
+
 def part_similarity(features: torch.Tensor, unit_queries: torch.Tensor, softmax_temperature: float = 0.1,
                     mask: Optional[torch.Tensor] = None, n_occupied: Optional[int] = None, with_probs: bool = True):
     """(similarities (N, P) fp32, labels (N,) int64, scores (N,) fp32, probabilities (N, P) fp32 or None) for the rows of the
-    float16 `features` (..., C) selected by the boolean `mask` (over the leading dims, C order; every row without one).
+    float16 `features` (..., C) selected by `mask` (over the leading dims, C order, any non-zero entry as in `mask.bool()`;
+    every row without one).
     `unit_queries` (P, C) fp32 are normalize_queries' rows. `n_occupied` is mask's count when the caller has it."""
     lib = _lib.require_device()
     if not features.is_cuda or features.dtype != torch.float16:
@@ -80,7 +87,7 @@ def part_similarity(features: torch.Tensor, unit_queries: torch.Tensor, softmax_
     q = unit_queries.to(dev, torch.float32).contiguous()
     m8 = None
     if mask is not None:
-        m8 = mask.to(dev).reshape(-1).to(torch.uint8).contiguous()
+        m8 = mask_flags(mask, dev)
         if m8.numel() != f.shape[0]:
             raise ValueError(f"mask has {m8.numel()} entries for {f.shape[0]} feature rows")
         n = int(m8.count_nonzero()) if n_occupied is None else int(n_occupied)
@@ -99,9 +106,14 @@ def part_similarity(features: torch.Tensor, unit_queries: torch.Tensor, softmax_
 
 
 def knn_label_vote(coords: torch.Tensor, labels: torch.Tensor, k: int = 200) -> torch.Tensor:
-    """For each point, the smallest of the most frequent labels among its k nearest points (itself included; fp64
-    distances, ties at the k-th distance to the lowest index), int64 on the device of `coords`."""
+    """For each point, the smallest of the most frequent labels among its k nearest points (itself included; ties at the
+    k-th distance to the lowest index), int64 on the device of `coords`. The coordinates are rounded to float32 first; the
+    squared distances are then exact fp64 on those float32 values, not on float64 input as given."""
+    if coords.ndim != 2 or coords.shape[1] != 3:
+        raise ValueError(f"coords must be (n, 3), got {tuple(coords.shape)}")
     n = coords.shape[0]
+    if tuple(labels.shape) != (n,):
+        raise ValueError(f"labels must be ({n},) for {n} points, got {tuple(labels.shape)}")
     if not 1 <= k <= n:
         raise ValueError(f"Expected n_neighbors <= n_samples_fit, but n_neighbors = {k}, n_samples_fit = {n}, n_samples = {n}"
                          if k > n else f"k must be >= 1, got {k}")
@@ -118,10 +130,15 @@ def knn_label_vote(coords: torch.Tensor, labels: torch.Tensor, k: int = 200) -> 
 
 
 def nearest_vertex(vertices: np.ndarray, queries: torch.Tensor) -> torch.Tensor:
-    """Index (int64, host) of the nearest float64 vertex of each float32 query by the fp64 distance, ties to the lowest."""
+    """Index (int64, host) of the nearest float64 vertex of each float32 query by the fp64 distance, ties to the lowest. A
+    vertex with a NaN or Inf coordinate is never chosen; a finite one is, even where its squared distance overflows. -1 for a
+    non-finite query or without finite vertices."""
+    vertices = np.ascontiguousarray(vertices, dtype=np.float64)
+    if vertices.ndim != 2 or vertices.shape[1] != 3 or queries.ndim != 2 or queries.shape[1] != 3:
+        raise ValueError(f"vertices and queries must be (n, 3) and (m, 3), got {vertices.shape} and {tuple(queries.shape)}")
     lib = _lib.require_device()
     dev = queries.device if queries.is_cuda else torch.device("cuda", torch.cuda.current_device())
-    v = torch.from_numpy(np.ascontiguousarray(vertices, dtype=np.float64)).to(dev)
+    v = torch.from_numpy(vertices).to(dev)
     q = queries.to(dev, torch.float32).contiguous()
     idx = torch.empty(q.shape[0], dtype=torch.int32, device=dev)
     with torch.cuda.device(dev):

@@ -284,11 +284,16 @@ def _check_similarity(feats, mask, table, T=0.1):
     m_dev = torch.from_numpy(mask).to(DEV)
     q = S.normalize_queries(torch.from_numpy(table), DEV)
     sims, labels, scores, probs = S.part_similarity(f_dev, q, T, mask=m_dev)
-    n = int(mask.sum())
+    check_outputs(f_dev.reshape(-1, C)[m_dev.reshape(-1)], table, T, sims, labels, scores, probs)
+
+
+def check_outputs(rows, table, T, sims, labels, scores, probs):
+    """part_similarity's outputs for the float16 feature rows (n, C) on the device against the fp64 oracle, the label rule
+    and torch's softmax of the kernel's similarities."""
+    n, C = rows.shape
     assert sims.shape == (n, table.shape[0]) and labels.dtype == torch.int64
     if n == 0:
         return
-    rows = f_dev.reshape(-1, C)[m_dev.reshape(-1)]
     s64, _, _, _ = O.similarities(rows, table, T)
     err = (sims.double() - s64).abs().max().item()
     assert err <= sim_bound(C), (err, sim_bound(C))
