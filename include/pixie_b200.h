@@ -150,6 +150,20 @@ int pixie_gaussian_ply_records(const float* pos_dev, const float* cov_dev, const
 int pixie_gaussian_checkpoint_decode(const void* table_dev, long long n, int row_bytes, const int* cols, int K, int has_threshold,
                                      float threshold, float* pos_dev, float* shs_dev, float* opacity_dev, float* cov_dev,
                                      long long* m_host, void* stream);
+/* pixie_gaussian_checkpoint_decode_scale_rot: the same table and columns, every row, as GaussianModel.load_ply then get_xyz,
+ * get_features, get_opacity, get_scaling and get_rotation give it (what gaussian-splatting's render.py hands the rasterizer):
+ * pos_dev [n][3], shs_dev [n][K][3] and opacity_dev [n] as pixie_gaussian_checkpoint_decode writes them, scales_dev [n][3] =
+ * exp(scale_j), rotations_dev [n][4] = rot / max(||rot||, 1e-12) (F.normalize; w x y z as stored). Stream-ordered, no host
+ * sync. */
+int pixie_gaussian_checkpoint_decode_scale_rot(const void* table_dev, long long n, int row_bytes, const int* cols, int K, float* pos_dev,
+                                               float* shs_dev, float* opacity_dev, float* scales_dev, float* rotations_dev, void* stream);
+/* pixie_image_metrics: PSNR and SSIM of one image pair as gaussian-splatting's metrics.py scores it (utils/image_utils.py psnr,
+ * utils/loss_utils.py ssim with its 11-tap sigma-1.5 window, zero padding 5, C1 = 0.01^2, C2 = 0.03^2). a_dev, b_dev:
+ * [height][width][3] uint8, read as k / 255 in float32. window_host: the normalised float32 1D window; the 2D window is its
+ * outer product, exact in fp64. out_dev [2] fp64 = {psnr (inf for identical images), ssim}, computed in fp64 and reduced in
+ * a fixed order (bit-identical on a repeat). One kernel launch, stream-ordered, no host sync. */
+int pixie_image_metrics(const uint8_t* a_dev, const uint8_t* b_dev, int height, int width, const float window_host[11], double* out_dev,
+                        void* stream);
 /* pixie_material_metrics: the evaluation of the material networks on labelled scenes, process_batch's metric code
  * (WG/trainer/inference_combined.py:108-170, compute_accuracy / masked_mean of pixie/training_utils.py:68-87) together with
  * the ground-truth normalisation of MaterialVoxelDataset.__getitem__ (WG/data_utils/my_data.py:160-240).
@@ -232,6 +246,15 @@ int pixie_gs_render(pixie_gs_renderer_t h, const float* means_dev, const float* 
                     const float proj_host[16], const float campos_host[3], float tan_fovx, float tan_fovy, int width, int height,
                     const float bg_host[3], float* image_dev, int* radii_dev, int* n_rendered_host, float* phase_ms_host,
                     void* stream);
+/* pixie_gs_render_scale_rot: one frame as pixie_gs_render draws it, with the covariances built in the preprocess from
+ * scales_dev [n][3] and rotations_dev [n][4] (unit quaternions w x y z) as forward.cu's computeCov3D builds them at
+ * scale_modifier 1, and the colours from shs_dev (required) as its computeColorFromSH evaluates them: what
+ * gaussian_renderer.render passes with PipelineParams' defaults (gaussian-splatting's render.py). */
+int pixie_gs_render_scale_rot(pixie_gs_renderer_t h, const float* means_dev, const float* scales_dev, const float* rotations_dev,
+                              const float* opacity_dev, const float* shs_dev, int sh_coeffs, int sh_degree, int n, const float view_host[16],
+                              const float proj_host[16], const float campos_host[3], float tan_fovx, float tan_fovy, int width, int height,
+                              const float bg_host[3], float* image_dev, int* radii_dev, int* n_rendered_host, float* phase_ms_host,
+                              void* stream);
 void pixie_gs_renderer_destroy(pixie_gs_renderer_t h);
 /* Number of kernel launches one forward() issues (for gpu_launches accounting) and algorithmic
  * FLOPs of one forward at batch 1 (2 * MACs of every Conv3d/Conv1d of the reference graph). */

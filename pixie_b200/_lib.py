@@ -98,6 +98,9 @@ _SIGNATURES = {
     "pixie_gaussian_ply_records": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "pixie_gaussian_checkpoint_decode": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_float, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong), C.c_void_p]),
+    "pixie_gaussian_checkpoint_decode_scale_rot": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_void_p,
+                                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pixie_image_metrics": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.c_void_p, C.c_void_p]),
     "pixie_material_metrics": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int64, C.POINTER(C.c_double),
                                          C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pixie_fill_density": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -112,6 +115,10 @@ _SIGNATURES = {
     "pixie_gs_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                   C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float, C.c_float, C.c_int, C.c_int,
                                   C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_float), C.c_void_p]),
+    "pixie_gs_render_scale_rot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                            C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float, C.c_float,
+                                            C.c_int, C.c_int, C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.POINTER(C.c_int),
+                                            C.POINTER(C.c_float), C.c_void_p]),
     "pixie_gs_renderer_destroy": (None, [C.c_void_p]),
     "pixie_mpm_set_active_count": (C.c_int, [C.c_void_p, C.c_int]),
     "pixie_mpm_grid_ptrs": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),

@@ -10,6 +10,7 @@
 #include "gs_render.cuh"
 #include "gs_ply.cuh"
 #include "gs_load.cuh"
+#include "image_metrics.cuh"
 #include "material_metrics.cuh"
 #include "part_segmentation.cuh"
 #include "workspace.cuh"
@@ -148,16 +149,14 @@ int pixie_gaussian_ply_records(const float* pos, const float* cov, const float* 
     if (require_device()) return 1;
     return check("gaussian_ply_records", pixie::gaussian_ply_records(pos, cov, shs, K, opacity, n, records, (cudaStream_t)stream));
 }
-int pixie_gaussian_checkpoint_decode(const void* table, long long n, int row_bytes, const int* cols, int K, int has_threshold, float threshold,
-                                     float* pos, float* shs, float* opacity, float* cov, long long* m_host, void* stream) {
-    if (!cols || !m_host || (n > 0 && (!table || !pos || !shs || !opacity || !cov))) return fail("null argument");
-    if (n < 0) return fail("gaussian_checkpoint_decode: negative row count");
-    if (K != 1 && K != 4 && K != 9 && K != 16) return fail("gaussian_checkpoint_decode: K must be 1, 4, 9 or 16 SH coefficients");
+// The checks both checkpoint decodes share: K, the row stride and the column offsets (cols [11 + 3K] bytes) into c.
+static int checkpoint_columns(const char* op, int row_bytes, const int* cols, int K, pixie::GsColumns& c) {
+    const std::string who(op);
+    if (K != 1 && K != 4 && K != 9 && K != 16) return fail(who + ": K must be 1, 4, 9 or 16 SH coefficients");
     if (row_bytes < 4 || row_bytes % 4 != 0 || row_bytes / 4 > pixie::kGsLoadMaxRowWords)
-        return fail("gaussian_checkpoint_decode: the row stride must be a multiple of 4 bytes, at most " +
-                       std::to_string(4 * pixie::kGsLoadMaxRowWords));
+        return fail(who + ": the row stride must be a multiple of 4 bytes, at most " + std::to_string(4 * pixie::kGsLoadMaxRowWords));
     const int row_words = row_bytes / 4, n_cols = 11 + 3 * K;
-    pixie::GsColumns c{};
+    c = pixie::GsColumns{};
     int* dst[59];
     int k = 0;
     for (int i = 0; i < 3; ++i) dst[k++] = &c.xyz[i];
@@ -168,12 +167,36 @@ int pixie_gaussian_checkpoint_decode(const void* table, long long n, int row_byt
     for (int i = 0; i < 4; ++i) dst[k++] = &c.rot[i];
     for (int i = 0; i < n_cols; ++i) {
         if (cols[i] < 0 || cols[i] % 4 != 0 || cols[i] / 4 >= row_words)
-            return fail("gaussian_checkpoint_decode: column " + std::to_string(i) + " is not a 4-byte aligned offset inside the row");
+            return fail(who + ": column " + std::to_string(i) + " is not a 4-byte aligned offset inside the row");
         *dst[i] = cols[i] / 4;
     }
+    return 0;
+}
+int pixie_gaussian_checkpoint_decode(const void* table, long long n, int row_bytes, const int* cols, int K, int has_threshold, float threshold,
+                                     float* pos, float* shs, float* opacity, float* cov, long long* m_host, void* stream) {
+    if (!cols || !m_host || (n > 0 && (!table || !pos || !shs || !opacity || !cov))) return fail("null argument");
+    if (n < 0) return fail("gaussian_checkpoint_decode: negative row count");
+    pixie::GsColumns c;
+    if (checkpoint_columns("gaussian_checkpoint_decode", row_bytes, cols, K, c)) return 1;
     if (require_device()) return 1;
-    return check("gaussian_checkpoint_decode", pixie::gaussian_checkpoint_decode(table, n, row_words, c, K, has_threshold, threshold, pos, shs, opacity,
-                                                                                 cov, m_host, (cudaStream_t)stream));
+    return check("gaussian_checkpoint_decode", pixie::gaussian_checkpoint_decode(table, n, row_bytes / 4, c, K, has_threshold, threshold, pos, shs,
+                                                                                 opacity, cov, m_host, (cudaStream_t)stream));
+}
+int pixie_gaussian_checkpoint_decode_scale_rot(const void* table, long long n, int row_bytes, const int* cols, int K, float* pos, float* shs,
+                                               float* opacity, float* scales, float* rotations, void* stream) {
+    if (!cols || (n > 0 && (!table || !pos || !shs || !opacity || !scales || !rotations))) return fail("null argument");
+    if (n < 0) return fail("gaussian_checkpoint_decode_scale_rot: negative row count");
+    pixie::GsColumns c;
+    if (checkpoint_columns("gaussian_checkpoint_decode_scale_rot", row_bytes, cols, K, c)) return 1;
+    if (require_device()) return 1;
+    return check("gaussian_checkpoint_decode_scale_rot", pixie::gaussian_checkpoint_decode_scale_rot(table, n, row_bytes / 4, c, K, pos, shs, opacity,
+                                                                                                     scales, rotations, (cudaStream_t)stream));
+}
+int pixie_image_metrics(const uint8_t* a, const uint8_t* b, int height, int width, const float window[11], double* out, void* stream) {
+    if (!a || !b || !window || !out) return fail("null argument");
+    if (height < 1 || width < 1 || (long long)height * width > 2147483647LL / 3) return fail("image_metrics: bad image size");
+    if (require_device()) return 1;
+    return check("image_metrics", pixie::image_metrics(a, b, height, width, window, out, (cudaStream_t)stream));
 }
 int pixie_material_metrics(const float* mat, int c_mat, const float* mask, const float* seg, int n_classes, const float* cont, int n,
                            int64_t voxels, const double* ranges, int background_id, float* gt, long long* counts, double* sums, void* stream) {
@@ -258,26 +281,49 @@ int pixie_gs_renderer_create(pixie_gs_renderer_t* out) {
     *out = pixie::gs_renderer_create();
     return *out ? 0 : 1;
 }
-int pixie_gs_render(pixie_gs_renderer_t h, const float* means, const float* cov, const float* opacity, const float* shs, int sh_coeffs,
-                    int sh_degree, const float* colors, int n, const float view[16], const float proj[16], const float campos[3],
-                    float tan_fovx, float tan_fovy, int width, int height, const float bg[3], float* image, int* radii, int* n_rendered,
-                    float* phase_ms, void* stream) {
+// The checks and argument block both rasterizer entry points share; the caller sets the covariance source.
+static int gs_render_args(pixie_gs_renderer_t h, const float* means, const float* opacity, const float* shs, int sh_coeffs, int sh_degree,
+                          int n, const float view[16], const float proj[16], const float campos[3], float tan_fovx, float tan_fovy,
+                          int width, int height, const float bg[3], float* image, int* radii, pixie::GsRenderArgs& a) {
     if (!h) return fail("null handle");
-    if (!view || !proj || !campos || !bg || !image || (n > 0 && (!means || !cov || !opacity || !radii || (!shs && !colors))))
-        return fail("null argument");
+    if (!view || !proj || !campos || !bg || !image || (n > 0 && (!means || !opacity || !radii))) return fail("null argument");
     if (n < 0) return fail("gs_render: negative Gaussian count");
     if (width < 1 || height < 1 || (long long)width * height > 2147483647LL) return fail("gs_render: bad image size");
     if (!(tan_fovx > 0.f) || !(tan_fovy > 0.f)) return fail("gs_render: tan(fov) must be positive");
     if (shs && (sh_degree < 0 || sh_degree > 3 || (sh_degree + 1) * (sh_degree + 1) > sh_coeffs))
         return fail("gs_render: need 0 <= sh_degree <= 3 and (sh_degree + 1)^2 <= sh_coeffs");
-    pixie::GsRenderArgs a{};
-    a.means = means; a.cov = cov; a.opacity = opacity; a.shs = shs; a.colors = shs ? nullptr : colors;
+    a = pixie::GsRenderArgs{};
+    a.means = means; a.opacity = opacity; a.shs = shs;
     a.n = n; a.sh_coeffs = sh_coeffs; a.sh_degree = sh_degree;
     std::memcpy(a.view, view, sizeof(a.view));
     std::memcpy(a.proj, proj, sizeof(a.proj));
     std::memcpy(a.campos, campos, sizeof(a.campos));
     std::memcpy(a.bg, bg, sizeof(a.bg));
     a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy; a.width = width; a.height = height; a.image = image; a.radii = radii;
+    return 0;
+}
+int pixie_gs_render(pixie_gs_renderer_t h, const float* means, const float* cov, const float* opacity, const float* shs, int sh_coeffs,
+                    int sh_degree, const float* colors, int n, const float view[16], const float proj[16], const float campos[3],
+                    float tan_fovx, float tan_fovy, int width, int height, const float bg[3], float* image, int* radii, int* n_rendered,
+                    float* phase_ms, void* stream) {
+    if (h && n > 0 && (!cov || (!shs && !colors))) return fail("null argument");
+    pixie::GsRenderArgs a;
+    if (gs_render_args(h, means, opacity, shs, sh_coeffs, sh_degree, n, view, proj, campos, tan_fovx, tan_fovy, width, height, bg, image,
+                       radii, a))
+        return 1;
+    a.cov = cov; a.colors = shs ? nullptr : colors;
+    return pixie::gs_render(h, a, n_rendered, phase_ms, (cudaStream_t)stream);
+}
+int pixie_gs_render_scale_rot(pixie_gs_renderer_t h, const float* means, const float* scales, const float* rotations, const float* opacity,
+                              const float* shs, int sh_coeffs, int sh_degree, int n, const float view[16], const float proj[16],
+                              const float campos[3], float tan_fovx, float tan_fovy, int width, int height, const float bg[3], float* image,
+                              int* radii, int* n_rendered, float* phase_ms, void* stream) {
+    if (h && n > 0 && (!scales || !rotations || !shs)) return fail("null argument");
+    pixie::GsRenderArgs a;
+    if (gs_render_args(h, means, opacity, shs, sh_coeffs, sh_degree, n, view, proj, campos, tan_fovx, tan_fovy, width, height, bg, image,
+                       radii, a))
+        return 1;
+    a.scales = scales; a.rotations = rotations;
     return pixie::gs_render(h, a, n_rendered, phase_ms, (cudaStream_t)stream);
 }
 void pixie_gs_renderer_destroy(pixie_gs_renderer_t h) { pixie::gs_renderer_destroy(h); }

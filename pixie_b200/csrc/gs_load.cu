@@ -1,6 +1,8 @@
 // Trained 3DGS checkpoint decode: GaussianModel.load_ply (gaussian-splatting/scene/gaussian_model.py:215-260) followed by
 // get_xyz / get_features / get_opacity / get_covariance (:27-31, :117-118 with utils/general_utils.py:64-110) and, when a
-// threshold is given, the opacity filter of gs_simulation.py:405. The mirror image of gs_ply.cu.
+// threshold is given, the opacity filter of gs_simulation.py:405. The mirror image of gs_ply.cu. The second decode,
+// gaussian_checkpoint_decode_scale_rot, stops before the covariance and returns get_scaling and get_rotation as
+// gaussian_renderer/__init__.py hands them to the rasterizer (render.py).
 //
 // The reference reads each column into numpy, copies it to the device as a float32 tensor and runs the activations as
 // separate torch ops. Here the vertex table goes to the device as it is in the file and one thread decodes one row. A
@@ -40,11 +42,13 @@ __global__ void __launch_bounds__(kRows) count_kernel(const float* __restrict__ 
     if (threadIdx.x == 0) counts[blockIdx.x] = c;
 }
 
-template <int K>
+// kScaleRot: write scales [.][3] = exp(scale) to `cov` and rotations [.][4] = F.normalize(rot) to `rot_out` instead of
+// the covariance
+template <int K, bool kScaleRot>
 __global__ void __launch_bounds__(kRows) decode_kernel(const float* __restrict__ table, long long n, int row_words, const GsColumns cols,
                                                        int has_threshold, float threshold, const long long* __restrict__ offsets,
                                                        float* __restrict__ pos, float* __restrict__ shs, float* __restrict__ opacity,
-                                                       float* __restrict__ cov) {
+                                                       float* __restrict__ cov, float* __restrict__ rot_out) {
     extern __shared__ __align__(16) float rows[];
     __shared__ int warp_base[kWarps];
     const long long first = (long long)blockIdx.x * kRows;
@@ -95,6 +99,19 @@ __global__ void __launch_bounds__(kRows) decode_kernel(const float* __restrict__
     float s[3];
 #pragma unroll
     for (int j = 0; j < 3; ++j) s[j] = expf(row[cols.scale[j]]);
+    if constexpr (kScaleRot) {
+        // F.normalize: r / max(||r||, 1e-12), the norm's sum of squares in index order without FMA
+        const float q0 = row[cols.rot[0]], q1 = row[cols.rot[1]], q2 = row[cols.rot[2]], q3 = row[cols.rot[3]];
+        float nrm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q0, q0), __fmul_rn(q1, q1)), __fmul_rn(q2, q2)), __fmul_rn(q3, q3)));
+        if (nrm < 1e-12f) nrm = 1e-12f;                  // clamp_min: a NaN norm stays NaN
+#pragma unroll
+        for (int j = 0; j < 3; ++j) cov[3 * m + j] = s[j];
+        rot_out[4 * m + 0] = __fdiv_rn(q0, nrm);
+        rot_out[4 * m + 1] = __fdiv_rn(q1, nrm);
+        rot_out[4 * m + 2] = __fdiv_rn(q2, nrm);
+        rot_out[4 * m + 3] = __fdiv_rn(q3, nrm);
+        return;
+    }
     // build_rotation: norm = sqrt(((r0 r0 + r1 r1) + r2 r2) + r3 r3), q = r / norm, R as general_utils.py:90-98 writes it
     const float r0 = row[cols.rot[0]], r1 = row[cols.rot[1]], r2 = row[cols.rot[2]], r3 = row[cols.rot[3]];
     const float norm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(r0, r0), __fmul_rn(r1, r1)), __fmul_rn(r2, r2)), __fmul_rn(r3, r3)));
@@ -130,13 +147,16 @@ __global__ void __launch_bounds__(kRows) decode_kernel(const float* __restrict__
     }
 }
 
-template <int K>
+template <int K, bool kScaleRot = false>
 cudaError_t launch_decode(const float* table, long long n, int row_words, const GsColumns& cols, int has_threshold, float threshold,
-                          const long long* offsets, float* pos, float* shs, float* opacity, float* cov, cudaStream_t st) {
+                          const long long* offsets, float* pos, float* shs, float* opacity, float* cov, cudaStream_t st,
+                          float* rot = nullptr) {
     const size_t smem = (size_t)kRows * row_words * sizeof(float);
-    if (smem > 48 * 1024) PIXIE_TRY(cudaFuncSetAttribute(decode_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (smem > 48 * 1024)
+        PIXIE_TRY(cudaFuncSetAttribute(decode_kernel<K, kScaleRot>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const long long blocks = (n + kRows - 1) / kRows;
-    decode_kernel<K><<<(unsigned)blocks, kRows, smem, st>>>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs, opacity, cov);
+    decode_kernel<K, kScaleRot><<<(unsigned)blocks, kRows, smem, st>>>(table, n, row_words, cols, has_threshold, threshold, offsets, pos, shs,
+                                                                       opacity, cov, rot);
     return cudaGetLastError();
 }
 
@@ -171,6 +191,18 @@ cudaError_t gaussian_checkpoint_decode(const void* table_v, long long n, int row
     if (has_threshold) PIXIE_TRY(cudaStreamSynchronize(st));
     else *m_host = n;
     return cudaSuccess;
+}
+
+cudaError_t gaussian_checkpoint_decode_scale_rot(const void* table_v, long long n, int row_words, const GsColumns& cols, int K, float* pos,
+                                                 float* shs, float* opacity, float* scales, float* rotations, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    const float* table = static_cast<const float*>(table_v);
+    switch (K) {
+        case 1: return launch_decode<1, true>(table, n, row_words, cols, 0, 0.f, nullptr, pos, shs, opacity, scales, st, rotations);
+        case 4: return launch_decode<4, true>(table, n, row_words, cols, 0, 0.f, nullptr, pos, shs, opacity, scales, st, rotations);
+        case 9: return launch_decode<9, true>(table, n, row_words, cols, 0, 0.f, nullptr, pos, shs, opacity, scales, st, rotations);
+        default: return launch_decode<16, true>(table, n, row_words, cols, 0, 0.f, nullptr, pos, shs, opacity, scales, st, rotations);
+    }
 }
 
 }  // namespace pixie

@@ -19,5 +19,10 @@ constexpr int kGsLoadMaxRowWords = 448;   // 128 staged rows of at most 448 word
 // are. K is 1, 4, 9 or 16 and 1 <= row_words <= kGsLoadMaxRowWords. Host-synchronises on `st` once when filtering.
 cudaError_t gaussian_checkpoint_decode(const void* table, long long n, int row_words, const GsColumns& cols, int K, int has_threshold,
                                        float threshold, float* pos, float* shs, float* opacity, float* cov, long long* m_host, cudaStream_t st);
+// The same table and columns, every row, decoded as GaussianModel.load_ply then get_xyz, get_features, get_opacity,
+// get_scaling and get_rotation give it: pos, shs and opacity as above, scales [n][3] = exp(scale_j), rotations [n][4] =
+// rot / max(||rot||, 1e-12) (F.normalize; w x y z as stored). Stream-ordered, no host sync.
+cudaError_t gaussian_checkpoint_decode_scale_rot(const void* table, long long n, int row_words, const GsColumns& cols, int K, float* pos,
+                                                 float* shs, float* opacity, float* scales, float* rotations, cudaStream_t st);
 
 }  // namespace pixie

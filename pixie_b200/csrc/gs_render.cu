@@ -1,8 +1,10 @@
 // Forward Gaussian-splatting rasterizer for sm_90a: the frames gs_simulation.py:573-631 renders with `--render_img`
-// (Inria's diff-gaussian-rasterization, scale_modifier 1, prefiltered false, precomputed 3D covariances).
+// (Inria's diff-gaussian-rasterization, scale_modifier 1, prefiltered false, precomputed 3D covariances), and the dataset
+// views gaussian-splatting's render.py renders (the same rasterizer fed scales and rotations instead of covariances).
 //
 //   preprocess  one thread per Gaussian: near cull (view z <= 0.2), EWA projection of the covariance (x/z, y/z clamped to
-//               1.3 tan(fov)), +0.3 on the 2D diagonal, conic, radius ceil(3 sqrt(lambda_max)), 16x16-tile rectangle, and
+//               1.3 tan(fov)), +0.3 on the 2D diagonal (the covariance given, or built from scale and rotation as
+//               forward.cu's computeCov3D builds it), conic, radius ceil(3 sqrt(lambda_max)), 16x16-tile rectangle, and
 //               the colour: spherical harmonics toward the camera as utils/render_utils.py:113-130 evaluates them (+0.5,
 //               clamped at 0), or the caller's colours. Writes one 48-byte record per Gaussian for the blend.
 //   binning     inclusive scan of the tile counts; one host sync for the total; one (tile << 32 | depth bits) key per
@@ -89,7 +91,30 @@ __device__ __forceinline__ float eval_sh(int deg, const float* sh, float x, floa
     return r;
 }
 
+// forward.cu's computeCov3D at scale_modifier 1: S = diag(scale), R from the quaternion (r = rot.x) written as glm's
+// column-major constructor lists it (so R here is the transpose of the usual rotation matrix), M = S R, Sigma = M^T M; the
+// upper triangle in forward.cu's order (Sigma[0][0], [0][1], [0][2], [1][1], [1][2], [2][2]).
+__device__ __forceinline__ void cov3d_from_scale_rot(const float* __restrict__ scale, const float* __restrict__ rot, float (&cov)[6]) {
+    const float S[3][3] = {{scale[0], 0.0f, 0.0f}, {0.0f, scale[1], 0.0f}, {0.0f, 0.0f, scale[2]}};
+    const float r = rot[0], x = rot[1], y = rot[2], z = rot[3];
+    const float R[3][3] = {{1.f - 2.f * (y * y + z * z), 2.f * (x * y - r * z), 2.f * (x * z + r * y)},
+                           {2.f * (x * y + r * z), 1.f - 2.f * (x * x + z * z), 2.f * (y * z - r * x)},
+                           {2.f * (x * z - r * y), 2.f * (y * z + r * x), 1.f - 2.f * (x * x + y * y)}};
+    float M[3][3], Mt[3][3], Sig[3][3];
+    mat3_mul(S, R, M);
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = 0; b < 3; ++b) Mt[a][b] = M[b][a];
+    mat3_mul(Mt, M, Sig);
+    cov[0] = Sig[0][0]; cov[1] = Sig[0][1]; cov[2] = Sig[0][2];
+    cov[3] = Sig[1][1]; cov[4] = Sig[1][2]; cov[5] = Sig[2][2];
+}
+
+// kScaleRot: the covariance comes from scales [n][3] and rotations [n][4] (computeCov3D) instead of cov3d [n][6]
+template <bool kScaleRot>
 __global__ void __launch_bounds__(256) gs_preprocess_kernel(const float* __restrict__ means, const float* __restrict__ cov3d,
+                                                            const float* __restrict__ scales, const float* __restrict__ rotations,
                                                             const float* __restrict__ opacity, const float* __restrict__ shs,
                                                             const float* __restrict__ colors, int n, int sh_coeffs, int deg,
                                                             Cam c, int* __restrict__ radii, float* __restrict__ depths,
@@ -121,7 +146,9 @@ __global__ void __launch_bounds__(256) gs_preprocess_kernel(const float* __restr
                            {0.0f, c.focal_y / tz, -(c.focal_y * ty) / (tz * tz)},
                            {0.0f, 0.0f, 0.0f}};
     const float Wm[3][3] = {{v[0], v[4], v[8]}, {v[1], v[5], v[9]}, {v[2], v[6], v[10]}};
-    const float* s = cov3d + 6 * i;
+    float built[6];
+    if constexpr (kScaleRot) cov3d_from_scale_rot(scales + 3 * i, rotations + 4 * i, built);
+    const float* s = kScaleRot ? built : cov3d + 6 * i;
     const float V[3][3] = {{s[0], s[1], s[2]}, {s[1], s[3], s[4]}, {s[2], s[4], s[5]}};
     float T[3][3], Tt[3][3], A[3][3], S[3][3];
     mat3_mul(Wm, J, T);
@@ -147,7 +174,8 @@ __global__ void __launch_bounds__(256) gs_preprocess_kernel(const float* __restr
 
     float rgb[3];
     if (shs != nullptr) {
-        // utils/render_utils.py:121-128: direction from the camera centre, normalised; +0.5, clamped at 0
+        // utils/render_utils.py:121-128: direction from the camera centre, normalised; +0.5, clamped at 0. forward.cu's
+        // computeColorFromSH evaluates the same expressions in the same order, so both entry points share this code.
         const float dx = px - c.campos[0], dy = py - c.campos[1], dz = pz - c.campos[2];
         const float len = sqrtf(dx * dx + dy * dy + dz * dz);
         const float ux = dx / len, uy = dy / len, uz = dz / len;
@@ -366,9 +394,12 @@ int render_frame(GsRenderer* r, const GsRenderArgs& a, int* n_rendered, float* p
     const bool timed = phase_ms != nullptr;
     auto mark = [&](int k) { return timed ? cudaEventRecord(r->ev[k], st) : cudaSuccess; };
     if ((e = mark(0)) != cudaSuccess) return fail("gs_render: phase event", e);
-    if (n > 0)
-        gs_preprocess_kernel<<<(n + 255) / 256, 256, 0, st>>>(a.means, a.cov, a.opacity, a.shs, a.colors, n, a.sh_coeffs, a.sh_degree, c,
-                                                             a.radii, r->depths, r->rec, r->touched);
+    if (n > 0 && a.cov)
+        gs_preprocess_kernel<false><<<(n + 255) / 256, 256, 0, st>>>(a.means, a.cov, nullptr, nullptr, a.opacity, a.shs, a.colors, n,
+                                                                    a.sh_coeffs, a.sh_degree, c, a.radii, r->depths, r->rec, r->touched);
+    else if (n > 0)
+        gs_preprocess_kernel<true><<<(n + 255) / 256, 256, 0, st>>>(a.means, nullptr, a.scales, a.rotations, a.opacity, a.shs, a.colors, n,
+                                                                   a.sh_coeffs, a.sh_degree, c, a.radii, r->depths, r->rec, r->touched);
     if ((e = mark(1)) != cudaSuccess) return fail("gs_render: phase event", e);
 
     unsigned long long total = 0;

@@ -1,4 +1,5 @@
-// Forward Gaussian-splatting rasterizer (the renderer gs_simulation.py:573-631 calls; see gs_render.cu).
+// Forward Gaussian-splatting rasterizer (the renderer gs_simulation.py:573-631 and gaussian-splatting's render.py call; see
+// gs_render.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include "../../include/pixie_b200.h"
@@ -9,7 +10,9 @@ using GsRenderer = pixie_gs_renderer_s;    // the C ABI's handle is the renderer
 
 struct GsRenderArgs {
     const float* means;      // [n][3]
-    const float* cov;        // [n][6] upper triangle: xx xy xz yy yz zz
+    const float* cov;        // [n][6] upper triangle: xx xy xz yy yz zz, or NULL (then scales and rotations)
+    const float* scales;     // [n][3], with cov NULL
+    const float* rotations;  // [n][4] unit quaternions w x y z, with cov NULL
     const float* opacity;    // [n]
     const float* shs;        // [n][sh_coeffs][3] or NULL (then colors)
     const float* colors;     // [n][3] or NULL (then shs)

@@ -2,6 +2,8 @@
 rasterizer (gs_simulation.py:573-631 with `--render_img`; the reference calls Inria's diff-gaussian-rasterization).
 
     rasterize(means3D, cov3D, opacity, camera, bg, shs=None, sh_degree=0, colors=None) -> (image (3, H, W), radii (N,))
+    rasterize_scale_rot(means3D, scales, rotations, opacity, camera, bg, shs, sh_degree)  the same frame from scales and
+                                                                           rotations, as render.py's views are drawn
     get_camera_view(cameras, default_camera_index, ...)                    utils/camera_view_utils.py:164-268
     get_center_view_worldspace_and_observant_coordinate(...)               utils/transformation_utils.py:143-166
     decode_camera_params(sim_params)                                       utils/decode_param.py:212-270
@@ -327,4 +329,63 @@ def rasterize(means3D: torch.Tensor, cov3D: torch.Tensor, opacity: torch.Tensor,
     upper-triangular (xx, xy, xz, yy, yz, zz), opacity (N,) or (N, 1), all float32 CUDA tensors; colours from shs
     (N, (D+1)^2 or more, 3) at degree sh_degree <= 3 toward the camera centre, or from colors (N, 3) as given; bg: 3 values."""
     image, radii, _ = _rasterize(means3D, cov3D, opacity, camera, bg, shs, sh_degree, colors)
+    return image, radii
+
+
+def _rasterize_scale_rot(means3D, scales, rotations, opacity, camera: Camera, bg, shs, sh_degree: int,
+                         phase_ms: Optional[list] = None) -> Tuple[torch.Tensor, torch.Tensor, int]:
+    if means3D.dim() != 2 or means3D.shape[1] != 3:
+        raise ValueError(f"means3D must be (N, 3), got {tuple(means3D.shape)}")
+    n = means3D.shape[0]
+    if tuple(scales.shape) != (n, 3):
+        raise ValueError(f"scales must be (N, 3) = ({n}, 3), got {tuple(scales.shape)}")
+    if tuple(rotations.shape) != (n, 4):
+        raise ValueError(f"rotations must be (N, 4) = ({n}, 4), got {tuple(rotations.shape)}")
+    if not (tuple(opacity.shape) == (n,) or tuple(opacity.shape) == (n, 1)):
+        raise ValueError(f"opacity must be (N,) or (N, 1) for N = {n}, got {tuple(opacity.shape)}")
+    if int(sh_degree) not in (0, 1, 2, 3):
+        raise ValueError(f"sh_degree must be 0..3, got {sh_degree}")
+    if shs.dim() != 3 or shs.shape[0] != n or shs.shape[2] != 3 or shs.shape[1] < (int(sh_degree) + 1) ** 2:
+        raise ValueError(f"shs must be (N, K, 3) with K >= (sh_degree + 1)^2 = {(int(sh_degree) + 1) ** 2}, got {tuple(shs.shape)}")
+    W, H = int(camera.image_width), int(camera.image_height)
+    if W < 1 or H < 1:
+        raise ValueError(f"camera image size must be positive, got {W} x {H}")
+    tensors = [means3D, scales, rotations, opacity, shs]
+    if not all(t.is_cuda for t in tensors):
+        raise _lib.PixieError("rasterize_scale_rot requires CUDA tensors; there is no CPU fallback")
+    dev = means3D.device
+    if any(t.device != dev for t in tensors):
+        raise ValueError("means3D, scales, rotations, opacity and shs must be on one device")
+    if any(t.dtype != torch.float32 for t in tensors):
+        raise ValueError("means3D, scales, rotations, opacity and shs must be float32")
+    m, sc, rot, s = (t.detach().contiguous() for t in (means3D, scales, rotations, shs))
+    o = opacity.detach().reshape(-1).contiguous()
+    view = _f32(camera.world_view_transform, 16, "world_view_transform")
+    proj = _f32(camera.full_proj_transform, 16, "full_proj_transform")
+    campos = _f32(camera.camera_center, 3, "camera_center")
+    bgc = _f32(bg, 3, "bg")
+    r = _renderer(dev)
+    n_rendered = C.c_int(0)
+    ms = (C.c_float * 5)() if phase_ms is not None else None
+    with torch.cuda.device(dev), r.lock:
+        image = torch.empty((3, H, W), dtype=torch.float32, device=dev)
+        radii = torch.empty((n,), dtype=torch.int32, device=dev)
+        _lib.check(r.lib.pixie_gs_render_scale_rot(
+            r.h, C.c_void_p(m.data_ptr()), C.c_void_p(sc.data_ptr()), C.c_void_p(rot.data_ptr()), C.c_void_p(o.data_ptr()),
+            C.c_void_p(s.data_ptr()), int(s.shape[1]), int(sh_degree), n, view, proj, campos,
+            math.tan(camera.FoVx * 0.5), math.tan(camera.FoVy * 0.5), W, H, bgc, C.c_void_p(image.data_ptr()),
+            C.c_void_p(radii.data_ptr()), C.byref(n_rendered), ms, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    if phase_ms is not None:
+        phase_ms[:] = list(ms)
+    return image, radii, n_rendered.value
+
+
+def rasterize_scale_rot(means3D: torch.Tensor, scales: torch.Tensor, rotations: torch.Tensor, opacity: torch.Tensor, camera: Camera,
+                        bg, shs: torch.Tensor, sh_degree: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """One frame as gaussian_renderer.render draws it with PipelineParams' defaults (gaussian-splatting's render.py):
+    (image (3, H, W) float32 RGB, unclamped; radii (N,) int32). The covariance is built in the rasterizer's preprocess from
+    scales (N, 3) and rotations (N, 4) (unit quaternions w x y z) as forward.cu's computeCov3D builds it at scale_modifier
+    1; colours from shs (N, (D+1)^2 or more, 3) at degree sh_degree as its computeColorFromSH evaluates them. All float32
+    CUDA tensors; opacity (N,) or (N, 1); bg: 3 values."""
+    image, radii, _ = _rasterize_scale_rot(means3D, scales, rotations, opacity, camera, bg, shs, sh_degree)
     return image, radii

@@ -7,7 +7,8 @@ plyfile, Warp or its compiled rasterizer.
   them; none of the files these loaders read is written that way).
 - `load_checkpoint` / `load_gaussians` decode `point_cloud/iteration_*/point_cloud.ply` on the device: the vertex table is
   read straight into a pinned buffer, copied once, and `pixie_gaussian_checkpoint_decode` produces pos, shs, opacity and
-  the covariance, optionally keeping only the rows above the opacity threshold. The Gaussian columns must be float32
+  the covariance, optionally keeping only the rows above the opacity threshold. `decode_checkpoint_ply_scale_rot` decodes
+  the same table to the activated scales and normalised rotations instead, for render.py's views. The Gaussian columns must be float32
   (a stated deviation: plyfile would convert other types).
 - `decode_param_json`, `generate_rotation_matrices`, `load_point_cloud`, `load_e_field_from_ply` and
   `find_e_field_epoch` restate utils/decode_param.py, utils/transformation_utils.py and gs_simulation.py.
@@ -116,14 +117,30 @@ def _checkpoint_columns(el: PlyElement, K: int) -> List[int]:
     return out
 
 
-def decode_checkpoint_ply(path: str, sh_degree: int = 3, opacity_threshold: Optional[float] = None, device="cuda:0") -> Dict[str, torch.Tensor]:
-    """pos (M, 3), shs (M, K, 3), opacity (M, 1) and cov (M, 6) of a Gaussian checkpoint PLY, decoded on the device; with
-    `opacity_threshold`, only the rows whose opacity is > float32(threshold), in file order (gs_simulation.py:405)."""
+def _checkpoint_layout(path: str, sh_degree: int) -> Tuple[PlyElement, int, List[int]]:
+    """The checkpoint's vertex element, K and column offsets; raises on a bad degree or file before any device work."""
     K = (int(sh_degree) + 1) ** 2
     if K not in (1, 4, 9, 16):
         raise ValueError(f"sh_degree must be 0..3, got {sh_degree}")
     el = read_ply(path)
-    cols = _checkpoint_columns(el, K)
+    return el, K, _checkpoint_columns(el, K)
+
+
+def _checkpoint_table(el: PlyElement, dev: torch.device) -> torch.Tensor:
+    """The vertex rows, read straight into a pinned buffer and copied to `dev` once."""
+    nbytes = el.count * el.dtype.itemsize
+    host = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
+    with open(el.path, "rb") as f:
+        f.seek(el.data_offset)
+        if nbytes and f.readinto(memoryview(host.numpy())) != nbytes:
+            raise ValueError(f"{el.path}: short read")
+    return host.to(dev, non_blocking=True)
+
+
+def decode_checkpoint_ply(path: str, sh_degree: int = 3, opacity_threshold: Optional[float] = None, device="cuda:0") -> Dict[str, torch.Tensor]:
+    """pos (M, 3), shs (M, K, 3), opacity (M, 1) and cov (M, 6) of a Gaussian checkpoint PLY, decoded on the device; with
+    `opacity_threshold`, only the rows whose opacity is > float32(threshold), in file order (gs_simulation.py:405)."""
+    el, K, cols = _checkpoint_layout(path, sh_degree)
     lib = _lib.require_device()
     dev = torch.device(device)
     n, stride = el.count, el.dtype.itemsize
@@ -131,12 +148,7 @@ def decode_checkpoint_ply(path: str, sh_degree: int = 3, opacity_threshold: Opti
     shs = torch.empty((n, K, 3), dtype=torch.float32, device=dev)
     opacity = torch.empty((n, 1), dtype=torch.float32, device=dev)
     cov = torch.empty((n, 6), dtype=torch.float32, device=dev)
-    host = torch.empty(n * stride, dtype=torch.uint8, pin_memory=True)
-    with open(path, "rb") as f:
-        f.seek(el.data_offset)
-        if n * stride and f.readinto(memoryview(host.numpy())) != n * stride:
-            raise ValueError(f"{path}: short read")
-    table = host.to(dev, non_blocking=True)
+    table = _checkpoint_table(el, dev)
     thr = 0.0 if opacity_threshold is None else float(np.float32(opacity_threshold))
     m = C.c_longlong(0)
     with torch.cuda.device(dev):
@@ -148,6 +160,28 @@ def decode_checkpoint_ply(path: str, sh_degree: int = 3, opacity_threshold: Opti
     table.record_stream(torch.cuda.current_stream(dev))
     M = m.value
     return {"pos": pos[:M], "shs": shs[:M], "opacity": opacity[:M], "cov": cov[:M]}
+
+
+def decode_checkpoint_ply_scale_rot(path: str, sh_degree: int = 3, device="cuda:0") -> Dict[str, torch.Tensor]:
+    """pos (N, 3), shs (N, K, 3), opacity (N, 1), scales (N, 3) and rotations (N, 4) of a Gaussian checkpoint PLY, decoded on
+    the device as GaussianModel.load_ply then get_xyz, get_features, get_opacity (sigmoid), get_scaling (exp) and
+    get_rotation (F.normalize, w x y z as stored) give them: what gaussian-splatting's render.py rasterizes. No opacity
+    filter; the same pinned read and single host-to-device copy as decode_checkpoint_ply."""
+    el, K, cols = _checkpoint_layout(path, sh_degree)
+    lib = _lib.require_device()
+    dev = torch.device(device)
+    n, stride = el.count, el.dtype.itemsize
+    table = _checkpoint_table(el, dev)
+    out = {"pos": torch.empty((n, 3), dtype=torch.float32, device=dev), "shs": torch.empty((n, K, 3), dtype=torch.float32, device=dev),
+           "opacity": torch.empty((n, 1), dtype=torch.float32, device=dev), "scales": torch.empty((n, 3), dtype=torch.float32, device=dev),
+           "rotations": torch.empty((n, 4), dtype=torch.float32, device=dev)}
+    with torch.cuda.device(dev):
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        _lib.check(lib.pixie_gaussian_checkpoint_decode_scale_rot(
+            C.c_void_p(table.data_ptr()), n, stride, (C.c_int * len(cols))(*cols), K,
+            *(C.c_void_p(out[k].data_ptr()) for k in ("pos", "shs", "opacity", "scales", "rotations")), stream))
+    table.record_stream(torch.cuda.current_stream(dev))
+    return out
 
 
 def search_for_max_iteration(folder: str) -> int:
