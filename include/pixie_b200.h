@@ -226,35 +226,32 @@ int pixie_knn_label_vote(const float* pos_dev, int n, const int64_t* labels_dev,
  * -1 for a non-finite query or when no vertex is finite. vert_dev [n][3], query_dev [m][3], index_dev [m] int32. */
 int pixie_nearest_vertex(const double* vert_dev, int n, const float* query_dev, int m, int* index_dev, void* stream);
 /* ---- Gaussian-splatting rasteriser, forward only (gs_simulation.py:573-631 with `--render_img`: Inria's
- * diff-gaussian-rasterization at scale_modifier 1, prefiltered false, precomputed 3D covariances).
+ * diff-gaussian-rasterization at scale_modifier 1, prefiltered false).
  * A renderer keeps its device buffers between frames and grows them when a frame needs more; once warm, a frame allocates
- * nothing. pixie_gs_render draws one frame on `stream`: means_dev [n][3], cov_dev [n][6] (upper triangle xx xy xz yy yz zz,
- * the solver's export order), opacity_dev [n]; colours from shs_dev [n][sh_coeffs][3] evaluated at degree sh_degree (<= 3,
- * (sh_degree + 1)^2 <= sh_coeffs) toward campos as utils/render_utils.py:113-130 does (+0.5, clamped at 0), or, when
- * shs_dev is NULL, colors_dev [n][3] as given. view / proj: world_view_transform and full_proj_transform as the reference
- * stores them (16 floats each, row-vector convention). image_dev [3][height][width] receives the unclamped RGB image over
- * bg, radii_dev [n] the screen radius (0 = culled). The call synchronises `stream` once, for the number of (Gaussian, tile)
- * pairs, which goes to *n_rendered_host (may be NULL). phase_ms_host, when not NULL, receives the times in ms of preprocess,
- * scan + keys, sort, ranges and blend (CUDA events; the call then synchronises a second time). The frame returns with its
- * sort and blend still running on `stream`; the next frame of the same renderer, on any stream, first waits for them, so
- * frames run in call order whatever streams they are drawn on. A renderer is not safe to call from two host threads at
- * once: callers serialise its calls. */
+ * nothing. pixie_gs_render draws one frame on `stream`: means_dev [n][3], opacity_dev [n], and one covariance source:
+ *   - cov_dev [n][6] (upper triangle xx xy xz yy yz zz, the solver's export order), with scales_dev and rotations_dev NULL;
+ *     colours from shs_dev, or, when shs_dev is NULL, colors_dev [n][3] as given;
+ *   - or scales_dev [n][3] and rotations_dev [n][4] (unit quaternions w x y z), with cov_dev and colors_dev NULL: the
+ *     covariances are built in the preprocess as forward.cu's computeCov3D builds them at scale_modifier 1, and the colours
+ *     come from shs_dev (required). This is what gaussian_renderer.render passes with PipelineParams' defaults
+ *     (gaussian-splatting's render.py).
+ * Any other combination is refused. shs_dev [n][sh_coeffs][3] is evaluated at degree sh_degree (<= 3,
+ * (sh_degree + 1)^2 <= sh_coeffs) toward campos as utils/render_utils.py:113-130 and computeColorFromSH do (+0.5, clamped
+ * at 0). view / proj: world_view_transform and full_proj_transform as the reference stores them (16 floats each,
+ * row-vector convention). image_dev [3][height][width] receives the unclamped RGB image over bg, radii_dev [n] the screen
+ * radius (0 = culled). The call synchronises `stream` once, for the number of (Gaussian, tile) pairs, which goes to
+ * *n_rendered_host (may be NULL). phase_ms_host, when not NULL, receives the times in ms of preprocess, scan + keys, sort,
+ * ranges and blend (CUDA events; the call then synchronises a second time). The frame returns with its sort and blend
+ * still running on `stream`; the next frame of the same renderer, on any stream, first waits for them, so frames run in
+ * call order whatever streams they are drawn on. A renderer is not safe to call from two host threads at once: callers
+ * serialise its calls. */
 typedef struct pixie_gs_renderer_s* pixie_gs_renderer_t;
 int pixie_gs_renderer_create(pixie_gs_renderer_t* out);
-int pixie_gs_render(pixie_gs_renderer_t h, const float* means_dev, const float* cov_dev, const float* opacity_dev,
-                    const float* shs_dev, int sh_coeffs, int sh_degree, const float* colors_dev, int n, const float view_host[16],
-                    const float proj_host[16], const float campos_host[3], float tan_fovx, float tan_fovy, int width, int height,
-                    const float bg_host[3], float* image_dev, int* radii_dev, int* n_rendered_host, float* phase_ms_host,
-                    void* stream);
-/* pixie_gs_render_scale_rot: one frame as pixie_gs_render draws it, with the covariances built in the preprocess from
- * scales_dev [n][3] and rotations_dev [n][4] (unit quaternions w x y z) as forward.cu's computeCov3D builds them at
- * scale_modifier 1, and the colours from shs_dev (required) as its computeColorFromSH evaluates them: what
- * gaussian_renderer.render passes with PipelineParams' defaults (gaussian-splatting's render.py). */
-int pixie_gs_render_scale_rot(pixie_gs_renderer_t h, const float* means_dev, const float* scales_dev, const float* rotations_dev,
-                              const float* opacity_dev, const float* shs_dev, int sh_coeffs, int sh_degree, int n, const float view_host[16],
-                              const float proj_host[16], const float campos_host[3], float tan_fovx, float tan_fovy, int width, int height,
-                              const float bg_host[3], float* image_dev, int* radii_dev, int* n_rendered_host, float* phase_ms_host,
-                              void* stream);
+int pixie_gs_render(pixie_gs_renderer_t h, const float* means_dev, const float* cov_dev, const float* scales_dev,
+                    const float* rotations_dev, const float* opacity_dev, const float* shs_dev, int sh_coeffs, int sh_degree,
+                    const float* colors_dev, int n, const float view_host[16], const float proj_host[16], const float campos_host[3],
+                    float tan_fovx, float tan_fovy, int width, int height, const float bg_host[3], float* image_dev, int* radii_dev,
+                    int* n_rendered_host, float* phase_ms_host, void* stream);
 void pixie_gs_renderer_destroy(pixie_gs_renderer_t h);
 /* Number of kernel launches one forward() issues (for gpu_launches accounting) and algorithmic
  * FLOPs of one forward at batch 1 (2 * MACs of every Conv3d/Conv1d of the reference graph). */

@@ -5,9 +5,11 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpixie_b200.so")
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 
 class PixieError(RuntimeError):
@@ -112,13 +114,10 @@ _SIGNATURES = {
     "pixie_knn_label_vote": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "pixie_nearest_vertex": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "pixie_gs_renderer_create": (C.c_int, [C.POINTER(C.c_void_p)]),
-    "pixie_gs_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
-                                  C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float, C.c_float, C.c_int, C.c_int,
-                                  C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_float), C.c_void_p]),
-    "pixie_gs_render_scale_rot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
-                                            C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float, C.c_float,
-                                            C.c_int, C.c_int, C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.POINTER(C.c_int),
-                                            C.POINTER(C.c_float), C.c_void_p]),
+    "pixie_gs_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                  C.c_void_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float,
+                                  C.c_float, C.c_int, C.c_int, C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.POINTER(C.c_int),
+                                  C.POINTER(C.c_float), C.c_void_p]),
     "pixie_gs_renderer_destroy": (None, [C.c_void_p]),
     "pixie_mpm_set_active_count": (C.c_int, [C.c_void_p, C.c_int]),
     "pixie_mpm_grid_ptrs": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
@@ -165,6 +164,28 @@ def last_error() -> PixieError:
 def check(rc: int):
     if rc != 0:
         raise last_error()
+
+
+def require_cuda(op: str, *tensors):
+    if not all(t.is_cuda for t in tensors):
+        raise PixieError(f"{op} requires CUDA tensors; there is no CPU fallback")
+
+
+def ptr(t):
+    """A tensor's device pointer as the library borrows it; None (a null pointer) for an absent array."""
+    return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def stream(dev) -> C.c_void_p:
+    """The current stream of `dev`, which every device operation takes as its last argument."""
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def call(name: str, dev, *args):
+    """Run the stateless device operation `name` on `dev`'s current stream: tensors are passed as borrowed pointers, every
+    other argument as given, and a non-zero return raises the library's message. Callers check the device themselves."""
+    with torch.cuda.device(dev):
+        check(getattr(load(), name)(*(ptr(a) if isinstance(a, torch.Tensor) else a for a in args), stream(dev)))
 
 
 def require_device():

@@ -41,7 +41,7 @@ int check(const char* op, cudaError_t e) { return e == cudaSuccess ? 0 : fail(op
 extern "C" {
 
 const char* pixie_last_error(void) { return g_err.c_str(); }
-int pixie_abi_version(void) { return 2; }
+int pixie_abi_version(void) { return 3; }
 
 int pixie_device_ok(void) {
     int dev = 0;
@@ -281,10 +281,14 @@ int pixie_gs_renderer_create(pixie_gs_renderer_t* out) {
     *out = pixie::gs_renderer_create();
     return *out ? 0 : 1;
 }
-// The checks and argument block both rasterizer entry points share; the caller sets the covariance source.
-static int gs_render_args(pixie_gs_renderer_t h, const float* means, const float* opacity, const float* shs, int sh_coeffs, int sh_degree,
-                          int n, const float view[16], const float proj[16], const float campos[3], float tan_fovx, float tan_fovy,
-                          int width, int height, const float bg[3], float* image, int* radii, pixie::GsRenderArgs& a) {
+int pixie_gs_render(pixie_gs_renderer_t h, const float* means, const float* cov, const float* scales, const float* rotations,
+                    const float* opacity, const float* shs, int sh_coeffs, int sh_degree, const float* colors, int n, const float view[16],
+                    const float proj[16], const float campos[3], float tan_fovx, float tan_fovy, int width, int height, const float bg[3],
+                    float* image, int* radii, int* n_rendered, float* phase_ms, void* stream) {
+    const bool scale_rot = scales || rotations;
+    if (cov && scale_rot) return fail("gs_render: give cov_dev or scales_dev and rotations_dev, not both");
+    if (scale_rot && colors) return fail("gs_render: colors_dev needs cov_dev; scales_dev and rotations_dev take shs_dev");
+    if (h && n > 0 && (scale_rot ? (!scales || !rotations || !shs) : (!cov || (!shs && !colors)))) return fail("null argument");
     if (!h) return fail("null handle");
     if (!view || !proj || !campos || !bg || !image || (n > 0 && (!means || !opacity || !radii))) return fail("null argument");
     if (n < 0) return fail("gs_render: negative Gaussian count");
@@ -292,38 +296,15 @@ static int gs_render_args(pixie_gs_renderer_t h, const float* means, const float
     if (!(tan_fovx > 0.f) || !(tan_fovy > 0.f)) return fail("gs_render: tan(fov) must be positive");
     if (shs && (sh_degree < 0 || sh_degree > 3 || (sh_degree + 1) * (sh_degree + 1) > sh_coeffs))
         return fail("gs_render: need 0 <= sh_degree <= 3 and (sh_degree + 1)^2 <= sh_coeffs");
-    a = pixie::GsRenderArgs{};
-    a.means = means; a.opacity = opacity; a.shs = shs;
+    pixie::GsRenderArgs a{};
+    a.means = means; a.cov = cov; a.scales = scales; a.rotations = rotations; a.opacity = opacity;
+    a.shs = shs; a.colors = shs ? nullptr : colors;
     a.n = n; a.sh_coeffs = sh_coeffs; a.sh_degree = sh_degree;
     std::memcpy(a.view, view, sizeof(a.view));
     std::memcpy(a.proj, proj, sizeof(a.proj));
     std::memcpy(a.campos, campos, sizeof(a.campos));
     std::memcpy(a.bg, bg, sizeof(a.bg));
     a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy; a.width = width; a.height = height; a.image = image; a.radii = radii;
-    return 0;
-}
-int pixie_gs_render(pixie_gs_renderer_t h, const float* means, const float* cov, const float* opacity, const float* shs, int sh_coeffs,
-                    int sh_degree, const float* colors, int n, const float view[16], const float proj[16], const float campos[3],
-                    float tan_fovx, float tan_fovy, int width, int height, const float bg[3], float* image, int* radii, int* n_rendered,
-                    float* phase_ms, void* stream) {
-    if (h && n > 0 && (!cov || (!shs && !colors))) return fail("null argument");
-    pixie::GsRenderArgs a;
-    if (gs_render_args(h, means, opacity, shs, sh_coeffs, sh_degree, n, view, proj, campos, tan_fovx, tan_fovy, width, height, bg, image,
-                       radii, a))
-        return 1;
-    a.cov = cov; a.colors = shs ? nullptr : colors;
-    return pixie::gs_render(h, a, n_rendered, phase_ms, (cudaStream_t)stream);
-}
-int pixie_gs_render_scale_rot(pixie_gs_renderer_t h, const float* means, const float* scales, const float* rotations, const float* opacity,
-                              const float* shs, int sh_coeffs, int sh_degree, int n, const float view[16], const float proj[16],
-                              const float campos[3], float tan_fovx, float tan_fovy, int width, int height, const float bg[3], float* image,
-                              int* radii, int* n_rendered, float* phase_ms, void* stream) {
-    if (h && n > 0 && (!scales || !rotations || !shs)) return fail("null argument");
-    pixie::GsRenderArgs a;
-    if (gs_render_args(h, means, opacity, shs, sh_coeffs, sh_degree, n, view, proj, campos, tan_fovx, tan_fovy, width, height, bg, image,
-                       radii, a))
-        return 1;
-    a.scales = scales; a.rotations = rotations;
     return pixie::gs_render(h, a, n_rendered, phase_ms, (cudaStream_t)stream);
 }
 void pixie_gs_renderer_destroy(pixie_gs_renderer_t h) { pixie::gs_renderer_destroy(h); }

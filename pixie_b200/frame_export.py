@@ -21,20 +21,15 @@ import torch
 from . import _lib
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def get_particle_volume(pos: torch.Tensor, grid_n: int, grid_dx: float, unifrom: bool = False) -> torch.Tensor:
     """vol[p] = grid_dx^3 / (number of particles in p's cell); with `unifrom` the mean volume for every particle (:282-285)."""
-    lib = _lib.require_device()
+    _lib.require_device()
     if not pos.is_cuda:
         raise _lib.PixieError("get_particle_volume requires a CUDA tensor; there is no CPU fallback")
     p = pos.detach().reshape(-1, 3).to(torch.float32).contiguous()
     n = p.shape[0]
-    with torch.cuda.device(p.device):
-        vol = torch.empty(n, dtype=torch.float32, device=p.device)
-        _lib.check(lib.pixie_particle_volume(C.c_void_p(p.data_ptr()), n, int(grid_n), float(grid_dx), C.c_void_p(vol.data_ptr()), _stream(p.device)))
+    vol = torch.empty(n, dtype=torch.float32, device=p.device)
+    _lib.call("pixie_particle_volume", p.device, p, n, int(grid_n), float(grid_dx), vol)
     if unifrom:
         return torch.mean(vol).repeat(n)
     return vol
@@ -43,9 +38,8 @@ def get_particle_volume(pos: torch.Tensor, grid_n: int, grid_dx: float, unifrom:
 def render_frame_transform(pos: torch.Tensor, cov: Optional[torch.Tensor], z_shift_value: float, scale_origin, original_mean_pos,
                            rotation_matrices: Sequence[torch.Tensor]) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """(pos_render, cov3D_render) of gs_simulation.py:594-598: simulation frame -> the Gaussians' original frame."""
-    lib = _lib.require_device()
-    if not pos.is_cuda:
-        raise _lib.PixieError("render_frame_transform requires CUDA tensors; there is no CPU fallback")
+    _lib.require_device()
+    _lib.require_cuda("render_frame_transform", pos)
     dev = pos.device
     p = pos.detach().reshape(-1, 3).to(torch.float32).contiguous()
     n = p.shape[0]
@@ -58,12 +52,9 @@ def render_frame_transform(pos: torch.Tensor, cov: Optional[torch.Tensor], z_shi
     if len(rots) > 8:
         raise ValueError("at most 8 rotation matrices")
     flat = (C.c_float * max(1, 9 * len(rots)))(*[v for r in rots for v in r])
-    with torch.cuda.device(dev):
-        po = torch.empty_like(p)
-        co = None if c is None else torch.empty_like(c)
-        _lib.check(lib.pixie_frame_transform(C.c_void_p(p.data_ptr()), C.c_void_p(c.data_ptr()) if c is not None else None, n, float(z_shift_value),
-                                             scale, (C.c_float * 3)(*mean), flat, len(rots), C.c_void_p(po.data_ptr()),
-                                             C.c_void_p(co.data_ptr()) if co is not None else None, _stream(dev)))
+    po = torch.empty_like(p)
+    co = None if c is None else torch.empty_like(c)
+    _lib.call("pixie_frame_transform", dev, p, c, n, float(z_shift_value), scale, (C.c_float * 3)(*mean), flat, len(rots), po, co)
     return po, co
 
 
@@ -93,9 +84,8 @@ def gaussian_ply_records(pos: torch.Tensor, cov: torch.Tensor, shs: torch.Tensor
     normals, shs[:, 0], shs[:, 1:] transposed to (3, K - 1) and flattened, opacity, the log scales and the (w, x, y, z)
     quaternion of cov3D_to_log_scales_and_quats. A covariance with a NaN or +-Inf entry gives NaN log scales and a NaN
     quaternion in its row; its other columns are copied as they are. One kernel, stream-ordered on the current stream."""
-    lib = _lib.require_device()
-    if not pos.is_cuda:
-        raise _lib.PixieError("gaussian_ply_records requires CUDA tensors; there is no CPU fallback")
+    _lib.require_device()
+    _lib.require_cuda("gaussian_ply_records", pos)
     dev = pos.device
     p = pos.detach().reshape(-1, 3).to(torch.float32).contiguous()
     n = p.shape[0]
@@ -107,10 +97,8 @@ def gaussian_ply_records(pos: torch.Tensor, cov: torch.Tensor, shs: torch.Tensor
     if c.shape[0] != n or s.shape[0] != n or o.shape[0] != n:
         raise ValueError(f"pos, cov, shs and opacity disagree on the Gaussian count ({n}, {c.shape[0]}, {s.shape[0]}, {o.shape[0]})")
     K = s.shape[1]
-    with torch.cuda.device(dev):
-        rec = torch.empty((n, 14 + 3 * K), dtype=torch.float32, device=dev)
-        _lib.check(lib.pixie_gaussian_ply_records(C.c_void_p(p.data_ptr()), C.c_void_p(c.data_ptr()), C.c_void_p(s.data_ptr()), K,
-                                                  C.c_void_p(o.data_ptr()), n, C.c_void_p(rec.data_ptr()), _stream(dev)))
+    rec = torch.empty((n, 14 + 3 * K), dtype=torch.float32, device=dev)
+    _lib.call("pixie_gaussian_ply_records", dev, p, c, s, K, o, n, rec)
     return rec
 
 

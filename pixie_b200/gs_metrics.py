@@ -54,15 +54,13 @@ def image_metrics(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] 
         raise ValueError(f"images must both be (H, W, 3), got {tuple(a.shape)} and {tuple(b.shape)}")
     if not (a.is_cuda and b.is_cuda) or a.device != b.device:
         raise _lib.PixieError("image_metrics requires CUDA tensors on one device; there is no CPU fallback")
-    lib = _lib.require_device()
+    _lib.require_device()
     if _WINDOW is None:
         _WINDOW = (C.c_float * 11)(*ssim_window().tolist())
     a, b = a.contiguous(), b.contiguous()
     if out is None:
         out = torch.empty(2, dtype=torch.float64, device=a.device)
-    with torch.cuda.device(a.device):
-        _lib.check(lib.pixie_image_metrics(C.c_void_p(a.data_ptr()), C.c_void_p(b.data_ptr()), int(a.shape[0]), int(a.shape[1]), _WINDOW,
-                                           C.c_void_p(out.data_ptr()), C.c_void_p(torch.cuda.current_stream(a.device).cuda_stream)))
+    _lib.call("pixie_image_metrics", a.device, a, b, int(a.shape[0]), int(a.shape[1]), _WINDOW, out)
     return out
 
 

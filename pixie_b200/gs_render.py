@@ -269,18 +269,28 @@ def _f32(values, n: int, name: str):
     return (C.c_float * n)(*v.tolist())
 
 
-def _rasterize(means3D, cov3D, opacity, camera: Camera, bg, shs=None, sh_degree: int = 0, colors=None,
-               phase_ms: Optional[list] = None) -> Tuple[torch.Tensor, torch.Tensor, int]:
+def _rasterize(means3D, opacity, camera: Camera, bg, shs=None, sh_degree: int = 0, colors=None, *, cov3D=None, scales=None,
+               rotations=None, phase_ms: Optional[list] = None) -> Tuple[torch.Tensor, torch.Tensor, int]:
+    """The frame of rasterize (given cov3D; colours from shs or colors) or rasterize_scale_rot (given scales and rotations;
+    colours from shs), with its number of (Gaussian, tile) pairs. `phase_ms`, when given, receives the five phase times."""
     if means3D.dim() != 2 or means3D.shape[1] != 3:
         raise ValueError(f"means3D must be (N, 3), got {tuple(means3D.shape)}")
     n = means3D.shape[0]
-    if tuple(cov3D.shape) != (n, 6):
-        raise ValueError(f"cov3D must be (N, 6) = ({n}, 6), got {tuple(cov3D.shape)}")
+    if cov3D is not None:
+        if tuple(cov3D.shape) != (n, 6):
+            raise ValueError(f"cov3D must be (N, 6) = ({n}, 6), got {tuple(cov3D.shape)}")
+        op, names, source = "rasterize", "means3D, cov3D, opacity and shs / colors", [cov3D]
+    else:
+        if tuple(scales.shape) != (n, 3):
+            raise ValueError(f"scales must be (N, 3) = ({n}, 3), got {tuple(scales.shape)}")
+        if tuple(rotations.shape) != (n, 4):
+            raise ValueError(f"rotations must be (N, 4) = ({n}, 4), got {tuple(rotations.shape)}")
+        op, names, source = "rasterize_scale_rot", "means3D, scales, rotations, opacity and shs", [scales, rotations]
     if not (tuple(opacity.shape) == (n,) or tuple(opacity.shape) == (n, 1)):
         raise ValueError(f"opacity must be (N,) or (N, 1) for N = {n}, got {tuple(opacity.shape)}")
-    if (shs is None) == (colors is None):
+    if cov3D is not None and (shs is None) == (colors is None):
         raise ValueError("give exactly one of shs and colors")
-    if shs is not None:
+    if colors is None:
         if int(sh_degree) not in (0, 1, 2, 3):
             raise ValueError(f"sh_degree must be 0..3, got {sh_degree}")
         if shs.dim() != 3 or shs.shape[0] != n or shs.shape[2] != 3 or shs.shape[1] < (int(sh_degree) + 1) ** 2:
@@ -290,17 +300,15 @@ def _rasterize(means3D, cov3D, opacity, camera: Camera, bg, shs=None, sh_degree:
     W, H = int(camera.image_width), int(camera.image_height)
     if W < 1 or H < 1:
         raise ValueError(f"camera image size must be positive, got {W} x {H}")
-    tensors = [means3D, cov3D, opacity, shs if shs is not None else colors]
-    if not all(t.is_cuda for t in tensors):
-        raise _lib.PixieError("rasterize requires CUDA tensors; there is no CPU fallback")
+    tensors = [means3D, *source, opacity, shs if shs is not None else colors]
+    _lib.require_cuda(op, *tensors)
     dev = means3D.device
     if any(t.device != dev for t in tensors):
-        raise ValueError("means3D, cov3D, opacity and shs / colors must be on one device")
+        raise ValueError(f"{names} must be on one device")
     if any(t.dtype != torch.float32 for t in tensors):
-        raise ValueError("means3D, cov3D, opacity and shs / colors must be float32")
-    m, c, o = means3D.detach().contiguous(), cov3D.detach().contiguous(), opacity.detach().reshape(-1).contiguous()
-    s = shs.detach().contiguous() if shs is not None else None
-    col = colors.detach().contiguous() if colors is not None else None
+        raise ValueError(f"{names} must be float32")
+    m, c, sc, rot, s, col = (None if t is None else t.detach().contiguous() for t in (means3D, cov3D, scales, rotations, shs, colors))
+    o = opacity.detach().reshape(-1).contiguous()
     view = _f32(camera.world_view_transform, 16, "world_view_transform")
     proj = _f32(camera.full_proj_transform, 16, "full_proj_transform")
     campos = _f32(camera.camera_center, 3, "camera_center")
@@ -308,15 +316,12 @@ def _rasterize(means3D, cov3D, opacity, camera: Camera, bg, shs=None, sh_degree:
     r = _renderer(dev)
     n_rendered = C.c_int(0)
     ms = (C.c_float * 5)() if phase_ms is not None else None
-    with torch.cuda.device(dev), r.lock:
-        image = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-        radii = torch.empty((n,), dtype=torch.int32, device=dev)
-        _lib.check(r.lib.pixie_gs_render(
-            r.h, C.c_void_p(m.data_ptr()), C.c_void_p(c.data_ptr()), C.c_void_p(o.data_ptr()),
-            C.c_void_p(s.data_ptr() if s is not None else None), int(s.shape[1]) if s is not None else 0, int(sh_degree),
-            C.c_void_p(col.data_ptr() if col is not None else None), n, view, proj, campos,
-            math.tan(camera.FoVx * 0.5), math.tan(camera.FoVy * 0.5), W, H, bgc, C.c_void_p(image.data_ptr()),
-            C.c_void_p(radii.data_ptr()), C.byref(n_rendered), ms, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    image = torch.empty((3, H, W), dtype=torch.float32, device=dev)
+    radii = torch.empty((n,), dtype=torch.int32, device=dev)
+    with r.lock:
+        _lib.call("pixie_gs_render", dev, r.h, m, c, sc, rot, o, s, int(s.shape[1]) if s is not None else 0, int(sh_degree), col, n,
+                  view, proj, campos, math.tan(camera.FoVx * 0.5), math.tan(camera.FoVy * 0.5), W, H, bgc, image, radii,
+                  C.byref(n_rendered), ms)
     if phase_ms is not None:
         phase_ms[:] = list(ms)
     return image, radii, n_rendered.value
@@ -328,56 +333,8 @@ def rasterize(means3D: torch.Tensor, cov3D: torch.Tensor, opacity: torch.Tensor,
     """One frame: (image (3, H, W) float32 RGB, unclamped; radii (N,) int32, 0 where culled). means3D (N, 3), cov3D (N, 6)
     upper-triangular (xx, xy, xz, yy, yz, zz), opacity (N,) or (N, 1), all float32 CUDA tensors; colours from shs
     (N, (D+1)^2 or more, 3) at degree sh_degree <= 3 toward the camera centre, or from colors (N, 3) as given; bg: 3 values."""
-    image, radii, _ = _rasterize(means3D, cov3D, opacity, camera, bg, shs, sh_degree, colors)
+    image, radii, _ = _rasterize(means3D, opacity, camera, bg, shs, sh_degree, colors, cov3D=cov3D)
     return image, radii
-
-
-def _rasterize_scale_rot(means3D, scales, rotations, opacity, camera: Camera, bg, shs, sh_degree: int,
-                         phase_ms: Optional[list] = None) -> Tuple[torch.Tensor, torch.Tensor, int]:
-    if means3D.dim() != 2 or means3D.shape[1] != 3:
-        raise ValueError(f"means3D must be (N, 3), got {tuple(means3D.shape)}")
-    n = means3D.shape[0]
-    if tuple(scales.shape) != (n, 3):
-        raise ValueError(f"scales must be (N, 3) = ({n}, 3), got {tuple(scales.shape)}")
-    if tuple(rotations.shape) != (n, 4):
-        raise ValueError(f"rotations must be (N, 4) = ({n}, 4), got {tuple(rotations.shape)}")
-    if not (tuple(opacity.shape) == (n,) or tuple(opacity.shape) == (n, 1)):
-        raise ValueError(f"opacity must be (N,) or (N, 1) for N = {n}, got {tuple(opacity.shape)}")
-    if int(sh_degree) not in (0, 1, 2, 3):
-        raise ValueError(f"sh_degree must be 0..3, got {sh_degree}")
-    if shs.dim() != 3 or shs.shape[0] != n or shs.shape[2] != 3 or shs.shape[1] < (int(sh_degree) + 1) ** 2:
-        raise ValueError(f"shs must be (N, K, 3) with K >= (sh_degree + 1)^2 = {(int(sh_degree) + 1) ** 2}, got {tuple(shs.shape)}")
-    W, H = int(camera.image_width), int(camera.image_height)
-    if W < 1 or H < 1:
-        raise ValueError(f"camera image size must be positive, got {W} x {H}")
-    tensors = [means3D, scales, rotations, opacity, shs]
-    if not all(t.is_cuda for t in tensors):
-        raise _lib.PixieError("rasterize_scale_rot requires CUDA tensors; there is no CPU fallback")
-    dev = means3D.device
-    if any(t.device != dev for t in tensors):
-        raise ValueError("means3D, scales, rotations, opacity and shs must be on one device")
-    if any(t.dtype != torch.float32 for t in tensors):
-        raise ValueError("means3D, scales, rotations, opacity and shs must be float32")
-    m, sc, rot, s = (t.detach().contiguous() for t in (means3D, scales, rotations, shs))
-    o = opacity.detach().reshape(-1).contiguous()
-    view = _f32(camera.world_view_transform, 16, "world_view_transform")
-    proj = _f32(camera.full_proj_transform, 16, "full_proj_transform")
-    campos = _f32(camera.camera_center, 3, "camera_center")
-    bgc = _f32(bg, 3, "bg")
-    r = _renderer(dev)
-    n_rendered = C.c_int(0)
-    ms = (C.c_float * 5)() if phase_ms is not None else None
-    with torch.cuda.device(dev), r.lock:
-        image = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-        radii = torch.empty((n,), dtype=torch.int32, device=dev)
-        _lib.check(r.lib.pixie_gs_render_scale_rot(
-            r.h, C.c_void_p(m.data_ptr()), C.c_void_p(sc.data_ptr()), C.c_void_p(rot.data_ptr()), C.c_void_p(o.data_ptr()),
-            C.c_void_p(s.data_ptr()), int(s.shape[1]), int(sh_degree), n, view, proj, campos,
-            math.tan(camera.FoVx * 0.5), math.tan(camera.FoVy * 0.5), W, H, bgc, C.c_void_p(image.data_ptr()),
-            C.c_void_p(radii.data_ptr()), C.byref(n_rendered), ms, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-    if phase_ms is not None:
-        phase_ms[:] = list(ms)
-    return image, radii, n_rendered.value
 
 
 def rasterize_scale_rot(means3D: torch.Tensor, scales: torch.Tensor, rotations: torch.Tensor, opacity: torch.Tensor, camera: Camera,
@@ -387,5 +344,5 @@ def rasterize_scale_rot(means3D: torch.Tensor, scales: torch.Tensor, rotations: 
     scales (N, 3) and rotations (N, 4) (unit quaternions w x y z) as forward.cu's computeCov3D builds it at scale_modifier
     1; colours from shs (N, (D+1)^2 or more, 3) at degree sh_degree as its computeColorFromSH evaluates them. All float32
     CUDA tensors; opacity (N,) or (N, 1); bg: 3 values."""
-    image, radii, _ = _rasterize_scale_rot(means3D, scales, rotations, opacity, camera, bg, shs, sh_degree)
+    image, radii, _ = _rasterize(means3D, opacity, camera, bg, shs, sh_degree, scales=scales, rotations=rotations)
     return image, radii

@@ -5,7 +5,6 @@ process_batch's forward + argmax (:122-126) and save_predictions' (3 + n_classes
 """
 from __future__ import annotations
 
-import ctypes as C
 import os
 from typing import Optional, Tuple
 
@@ -69,9 +68,7 @@ class MaterialFieldPredictor:
         n, G = seg_logits.shape[0], self.grid_size
         if out is None:
             out = torch.empty((n, 3 + self.n_classes, G, G, G), dtype=torch.float32, device=self.device)
-        st = torch.cuda.current_stream(self.device).cuda_stream
-        _lib.check(_lib.load().pixie_pack_predictions(C.c_void_p(seg_logits.data_ptr()), C.c_void_p(cont_pred.data_ptr()),
-                                                      C.c_void_p(out.data_ptr()), n, G ** 3, self.n_classes, C.c_void_p(st)))
+        _lib.call("pixie_pack_predictions", self.device, seg_logits, cont_pred, out, n, G ** 3, self.n_classes)
         return out
 
     def check(self):

@@ -34,14 +34,6 @@ DEFAULT_RANGES = dict(density_min=1.703, density_max=3.871, E_min=3.018, E_max=1
 DEFAULT_VALUES = {"density": 1000.0, "E": 5000.0, "nu": 0.3, "part_label": 0, "material_id": "stationary"}
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
-def _ptr(t: torch.Tensor):
-    return C.c_void_p(t.data_ptr())
-
-
 def extract_material_points(pred: torch.Tensor, mask: torch.Tensor, min_bounds: Sequence[float], max_bounds: Sequence[float],
                             ranges: Optional[Dict[str, float]] = None) -> Dict[str, torch.Tensor]:
     """`unscale_prediction` + the vertex table of `map_pred_to_ply` (map_pred_to_coords.py:41-75, 198-245).
@@ -49,29 +41,26 @@ def extract_material_points(pred: torch.Tensor, mask: torch.Tensor, min_bounds: 
     pred: (3 + n_classes, D, D, D) float32 cuda — 3 continuous channels in ~[-1, 1] followed by class scores / one-hot;
     mask: (D, D, D), occupied where > 0. Returns the `params` dict PG/material_field.py works on: pos (M,3), density, E, nu,
     material_id, part_labels (= material_id, map_pred_to_coords.py:232), conf — device tensors, voxels in C order."""
-    lib = _lib.require_device()
+    _lib.require_device()
     r = dict(DEFAULT_RANGES if ranges is None else ranges)
     if pred.dim() != 4 or pred.shape[1] != pred.shape[2] or pred.shape[2] != pred.shape[3] or pred.shape[0] < 4:
         raise ValueError(f"pred must be (3 + n_classes, D, D, D), got {tuple(pred.shape)}")
     D, K = int(pred.shape[1]), int(pred.shape[0]) - 3
     if tuple(mask.shape) != (D, D, D):
         raise ValueError(f"Mask shape {tuple(mask.shape)} does not match grid shape {(D, D, D)}")      # map_pred_to_coords.py:190-191
-    if not pred.is_cuda:
-        raise _lib.PixieError("extract_material_points requires CUDA tensors; there is no CPU fallback")
+    _lib.require_cuda("extract_material_points", pred)
     dev = pred.device
     pred = pred.detach().to(torch.float32).contiguous()
     maskf = mask.detach().to(dev, torch.float32).contiguous()
     n = D ** 3
-    with torch.cuda.device(dev):
-        pos = torch.empty((n, 3), dtype=torch.float32, device=dev)
-        dens, E, nu, conf = (torch.empty(n, dtype=torch.float32, device=dev) for _ in range(4))
-        mat = torch.empty(n, dtype=torch.int32, device=dev)
-        rng = (C.c_double * 6)(r["density_min"], r["density_max"], r["E_min"], r["E_max"], r["nu_min"], r["nu_max"])
-        bmin = (C.c_double * 3)(*[float(v) for v in min_bounds])
-        bmax = (C.c_double * 3)(*[float(v) for v in max_bounds])
-        cnt = C.c_int(0)
-        _lib.check(lib.pixie_field_extract(_ptr(pred), K, _ptr(maskf), D, rng, bmin, bmax, _ptr(pos), _ptr(dens), _ptr(E), _ptr(nu), _ptr(mat),
-                                           _ptr(conf), C.byref(cnt), _stream(dev)))
+    pos = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    dens, E, nu, conf = (torch.empty(n, dtype=torch.float32, device=dev) for _ in range(4))
+    mat = torch.empty(n, dtype=torch.int32, device=dev)
+    rng = (C.c_double * 6)(r["density_min"], r["density_max"], r["E_min"], r["E_max"], r["nu_min"], r["nu_max"])
+    bmin = (C.c_double * 3)(*[float(v) for v in min_bounds])
+    bmax = (C.c_double * 3)(*[float(v) for v in max_bounds])
+    cnt = C.c_int(0)
+    _lib.call("pixie_field_extract", dev, pred, K, maskf, D, rng, bmin, bmax, pos, dens, E, nu, mat, conf, C.byref(cnt))
     m = cnt.value
     return {"pos": pos[:m], "density": dens[:m], "E": E[:m], "nu": nu[:m], "material_id": mat[:m], "part_labels": mat[:m].clone(),
             "conf": conf[:m]}
@@ -90,9 +79,8 @@ def perform_knn_smoothing(query_positions: torch.Tensor, params: Dict[str, torch
     m = int(params["pos"].shape[0])
     if int(k_smoothing_neighbors) > m:                                              # NearestNeighbors.kneighbors raises here too
         raise ValueError(f"Expected n_neighbors <= n_samples_fit, but n_neighbors = {k_smoothing_neighbors}, n_samples_fit = {m}")
-    lib = _lib.require_device()
-    if not query_positions.is_cuda:
-        raise _lib.PixieError("perform_knn_smoothing requires CUDA tensors; there is no CPU fallback")
+    _lib.require_device()
+    _lib.require_cuda("perform_knn_smoothing", query_positions)
     dev = query_positions.device
     f = lambda t: t.detach().to(dev, torch.float32).contiguous()
     i = lambda t: t.detach().to(dev, torch.int32).contiguous()
@@ -102,14 +90,12 @@ def perform_knn_smoothing(query_positions: torch.Tensor, params: Dict[str, torch
     # get_defaults (:38-50): mean of each continuous property, "stationary" material, part label 0
     mean = lambda t, key: float(t.mean().item()) if m > 0 else float(DEFAULT_VALUES.get(key, 0.0))
     defaults = (C.c_float * 4)(mean(dens, "density"), mean(E, "E"), mean(nu, "nu"), mean(conf, "conf"))
-    with torch.cuda.device(dev):
-        o_d, o_E, o_nu, o_c = (torch.empty(n_particles, dtype=torch.float32, device=dev) for _ in range(4))
-        o_m, o_p = (torch.empty(n_particles, dtype=torch.int32, device=dev) for _ in range(2))
-        too_far = C.c_int(0)
-        _lib.check(lib.pixie_knn_assign(_ptr(q), n_particles, _ptr(pos), _ptr(dens), _ptr(E), _ptr(nu), _ptr(mat), _ptr(part), _ptr(conf), m,
-                                        int(k_smoothing_neighbors), float(nn_distance_threshold), int(bool(weighted_assignment)), defaults,
-                                        int(get_material_name("stationary")), int(DEFAULT_VALUES["part_label"]),
-                                        _ptr(o_d), _ptr(o_E), _ptr(o_nu), _ptr(o_m), _ptr(o_p), _ptr(o_c), C.byref(too_far), _stream(dev)))
+    o_d, o_E, o_nu, o_c = (torch.empty(n_particles, dtype=torch.float32, device=dev) for _ in range(4))
+    o_m, o_p = (torch.empty(n_particles, dtype=torch.int32, device=dev) for _ in range(2))
+    too_far = C.c_int(0)
+    _lib.call("pixie_knn_assign", dev, q, n_particles, pos, dens, E, nu, mat, part, conf, m, int(k_smoothing_neighbors),
+              float(nn_distance_threshold), int(bool(weighted_assignment)), defaults, int(get_material_name("stationary")),
+              int(DEFAULT_VALUES["part_label"]), o_d, o_E, o_nu, o_m, o_p, o_c, C.byref(too_far))
     n_too_far = too_far.value
     print(f"Particles too far from nearest neighbor: {n_too_far}, Assigned: {n_particles - n_too_far}")
     assert n_too_far <= 0.1 * n_particles, (f"[CRITICAL] More than 10% of particles are too far from nearest neighbor. "
@@ -150,7 +136,7 @@ def _dbscan(positions: torch.Tensor, eps: float, min_samples: int, select: Optio
         raise ValueError(f"eps must be > 0, got {eps}")
     if int(min_samples) < 1:
         raise ValueError(f"min_samples must be >= 1, got {min_samples}")
-    lib = _lib.require_device()
+    _lib.require_device()
     if not torch.is_tensor(positions) or not positions.is_cuda:
         raise _lib.PixieError("dbscan requires CUDA tensors; there is no CPU fallback")
     dev = positions.device
@@ -161,25 +147,20 @@ def _dbscan(positions: torch.Tensor, eps: float, min_samples: int, select: Optio
         ids = torch.as_tensor(select).detach().reshape(-1).to(dev, torch.int32).contiguous()
         if ids.numel() != n:
             raise ValueError(f"select has {ids.numel()} entries for {n} points")
-    with torch.cuda.device(dev):
-        index = torch.empty(n, dtype=torch.int32, device=dev)
-        labels = torch.empty(n, dtype=torch.int32, device=dev)
-        m, k = C.c_int(0), C.c_int(0)
-        _lib.check(lib.pixie_dbscan(_ptr(p), n, None if ids is None else _ptr(ids), int(select_id), float(eps), int(min_samples),
-                                    _ptr(index), _ptr(labels), C.byref(m), C.byref(k), _stream(dev)))
+    index = torch.empty(n, dtype=torch.int32, device=dev)
+    labels = torch.empty(n, dtype=torch.int32, device=dev)
+    m, k = C.c_int(0), C.c_int(0)
+    _lib.call("pixie_dbscan", dev, p, n, ids, int(select_id), float(eps), int(min_samples), index, labels, C.byref(m), C.byref(k))
     return labels[:m.value], index[:m.value], k.value
 
 
 def _cluster_stats(positions: torch.Tensor, index: torch.Tensor, labels: torch.Tensor, n_clusters: int):
     """Host float32 / int arrays: (sizes [K], bbox_min [K, 3], bbox_max [K, 3]) of the clusters `_dbscan` found."""
-    lib = _lib.load()
     dev = positions.device
     p = positions.detach().reshape(-1, 3).to(torch.float32).contiguous()
-    with torch.cuda.device(dev):
-        sizes = torch.empty(n_clusters, dtype=torch.int32, device=dev)
-        lo, hi = (torch.empty((n_clusters, 3), dtype=torch.float32, device=dev) for _ in range(2))
-        _lib.check(lib.pixie_cluster_stats(_ptr(p), _ptr(index), _ptr(labels), int(labels.numel()), int(n_clusters), _ptr(sizes), _ptr(lo),
-                                           _ptr(hi), _stream(dev)))
+    sizes = torch.empty(n_clusters, dtype=torch.int32, device=dev)
+    lo, hi = (torch.empty((n_clusters, 3), dtype=torch.float32, device=dev) for _ in range(2))
+    _lib.call("pixie_cluster_stats", dev, p, index, labels, int(labels.numel()), int(n_clusters), sizes, lo, hi)
     return sizes.cpu().numpy(), lo.cpu().numpy(), hi.cpu().numpy()
 
 

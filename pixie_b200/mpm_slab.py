@@ -68,9 +68,6 @@ class FusedSlabBackend:
         self._active = -1
         self.set_active(n_active)
 
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
     # -- exchange set-up
     def export_handle(self) -> bytes:
         """64-byte cudaIpc handle of the exchange buffer, for a neighbour in another process."""
@@ -100,7 +97,7 @@ class FusedSlabBackend:
     # -- substep phases (each only enqueues kernels)
     def _phase(self, ph: int, dt: float):
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.pixie_mpm_slab_phase(self.solver._handle, ph, float(dt), self._stream()))
+            _lib.check(self.lib.pixie_mpm_slab_phase(self.solver._handle, ph, float(dt), _lib.stream(self.device)))
 
     def scatter(self, dt: float):
         self._phase(0, dt)
@@ -127,7 +124,7 @@ class FusedSlabBackend:
         over the sorted positions; no write-back of the particle fields, no host sync)."""
         out = torch.zeros(1, dtype=torch.int32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.pixie_mpm_slab_excursion(self.solver._handle, C.c_void_p(out.data_ptr()), self._stream()))
+            _lib.check(self.lib.pixie_mpm_slab_excursion(self.solver._handle, _lib.ptr(out), _lib.stream(self.device)))
         return out
 
     # -- particles

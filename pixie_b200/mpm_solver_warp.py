@@ -235,7 +235,7 @@ class MPM_Simulator_WARP:
             pass
 
     def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self._device).cuda_stream)
+        return _lib.stream(self._device)
 
     def _fence(self, write_back=True):
         """Puts a call that changes bindings, parameters, boundary conditions or the clock behind the substeps queued on
@@ -261,7 +261,7 @@ class MPM_Simulator_WARP:
     def _bind(self, fid: str, t: torch.Tensor):
         self._tensors[fid] = t
         self._fence()
-        _lib.check(_lib.load().pixie_mpm_bind(self._handle, _lib.FIELDS[fid], C.c_void_p(t.data_ptr())))
+        _lib.check(_lib.load().pixie_mpm_bind(self._handle, _lib.FIELDS[fid], _lib.ptr(t)))
 
     def _push_params(self):
         m = self.mpm_model
@@ -390,7 +390,7 @@ class MPM_Simulator_WARP:
         the per-box `apply_additional_params` launches (:436-452) + the mass update (:454-463) without a Python dict per box."""
         lib = _lib.load()
         b = boxes.detach().to(self._device, torch.float32).contiguous()
-        _lib.check(lib.pixie_mpm_apply_additional_params(self._handle, C.c_void_p(b.data_ptr()), int(b.shape[0]), self._stream()))
+        _lib.check(lib.pixie_mpm_apply_additional_params(self._handle, _lib.ptr(b), int(b.shape[0]), self._stream()))
         _lib.check(lib.pixie_mpm_compute_mass(self._handle, self._stream()))
 
     def finalize_mu_lam(self, device="cuda:0"):
@@ -488,7 +488,7 @@ class MPM_Simulator_WARP:
         bc.translation_scale = float(kw.get("translation_scale", 0.0))
         if mask is not None:
             self._masks.append(mask)
-            bc.mask_dev = C.c_void_p(mask.data_ptr())
+            bc.mask_dev = _lib.ptr(mask)
         self._fence()
         _lib.check(_lib.load().pixie_mpm_add_bc(self._handle, C.byref(bc)))
         self.n_bcs += 1
@@ -497,7 +497,7 @@ class MPM_Simulator_WARP:
     def _select_box(self, point, size) -> torch.Tensor:
         mask = torch.zeros(self.n_particles, dtype=torch.int32, device=self._device)
         p3, s3 = (C.c_float * 3)(*[float(v) for v in point]), (C.c_float * 3)(*[float(v) for v in size])
-        _lib.check(_lib.load().pixie_mpm_select_box(self._handle, p3, s3, C.c_void_p(mask.data_ptr()), self._stream()))
+        _lib.check(_lib.load().pixie_mpm_select_box(self._handle, p3, s3, _lib.ptr(mask), self._stream()))
         return mask
 
     def add_surface_collider(self, point, normal, surface="sticky", friction=0.0, start_time=0.0, end_time=999.0):
@@ -552,8 +552,7 @@ class MPM_Simulator_WARP:
         mask = torch.zeros(self.n_particles, dtype=torch.int32, device=self._device)
         p3, n3 = (C.c_float * 3)(*[float(v) for v in point]), (C.c_float * 3)(*[float(v) for v in n])
         _lib.check(_lib.load().pixie_mpm_select_cylinder(self._handle, p3, n3, float(half_height_and_radius[0]),
-                                                         float(half_height_and_radius[1]), C.c_void_p(mask.data_ptr()),
-                                                         self._stream()))
+                                                         float(half_height_and_radius[1]), _lib.ptr(mask), self._stream()))
         bc = self._add_bc(_lib.BC_VELOCITY_ROTATION, mask=mask, point=point, normal=n, horizontal_axis_1=h1,
                           horizontal_axis_2=h2, half_height_and_radius=half_height_and_radius,
                           rotation_scale=rotation_scale, translation_scale=translation_scale, start_time=start_time,

@@ -178,9 +178,8 @@ def material_metrics(mat: torch.Tensor, mask: Optional[torch.Tensor], seg_logits
     (N, D, D, D) or None (then mask = id != background_id, compute_accuracy's other branch), seg_logits (N, K, D, D, D),
     cont_pred (N, 3, D, D, D), all float32 on one CUDA device. Returns (gt (N, 4, D, D, D) device, counts (N, 2) int64
     numpy = (total, correct), sums (N, 4) float64 numpy = (sum (cont - gt)^2 mask per channel, sum mask))."""
-    lib = _lib.require_device()
-    if not seg_logits.is_cuda:
-        raise _lib.PixieError("material_metrics requires CUDA tensors; there is no CPU fallback")
+    _lib.require_device()
+    _lib.require_cuda("material_metrics", seg_logits)
     dev = seg_logits.device
     n, K = int(seg_logits.shape[0]), int(seg_logits.shape[1])
     spatial = tuple(seg_logits.shape[2:])
@@ -192,16 +191,14 @@ def material_metrics(mat: torch.Tensor, mask: Optional[torch.Tensor], seg_logits
     f = lambda t: t.detach().to(dev, torch.float32).contiguous()                        # noqa: E731
     mat_, seg_, cont_ = f(mat), f(seg_logits), f(cont_pred)
     mask_ = None if mask is None else f(mask)
-    with torch.cuda.device(dev):
-        gt = gt_out if gt_out is not None else torch.empty((n, 4) + spatial, dtype=torch.float32, device=dev)
-        counts = torch.empty((n, 2), dtype=torch.int64, device=dev)
-        sums = torch.empty((n, 4), dtype=torch.float64, device=dev)
-        r = ranges
-        rng = (C.c_double * 6)(r["density_min"], r["density_max"], r["E_min"], r["E_max"], r["nu_min"], r["nu_max"])
-        p = lambda t: C.c_void_p(None if t is None else t.data_ptr())                   # noqa: E731
-        _lib.check(lib.pixie_material_metrics(p(mat_), int(mat.shape[-1]), p(mask_), p(seg_), K, p(cont_), n, V, rng, int(background_id),
-                                              p(gt), p(counts), p(sums), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-        return gt, counts.cpu().numpy(), sums.cpu().numpy()
+    gt = gt_out if gt_out is not None else torch.empty((n, 4) + spatial, dtype=torch.float32, device=dev)
+    counts = torch.empty((n, 2), dtype=torch.int64, device=dev)
+    sums = torch.empty((n, 4), dtype=torch.float64, device=dev)
+    r = ranges
+    rng = (C.c_double * 6)(r["density_min"], r["density_max"], r["E_min"], r["E_max"], r["nu_min"], r["nu_max"])
+    _lib.call("pixie_material_metrics", dev, mat_, int(mat.shape[-1]), mask_, seg_, K, cont_, n, V, rng, int(background_id), gt, counts,
+              sums)
+    return gt, counts.cpu().numpy(), sums.cpu().numpy()
 
 
 def _accuracy(total: int, correct: int) -> float:

@@ -30,10 +30,6 @@ from . import _lib
 _DIRS = "0: +x, 1: -x, 2: +y, 3: -y, 4: +z, 5: -z"
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def decode_filling_params(filling: Dict, material_params: Dict) -> Dict:
     """The `particle_filling` block of a physics config with the defaults of decode_param.py:177-208 (a new dict; the
     reference fills them in place). `max_partciels_per_cell` is the reference's own spelling of the key."""
@@ -60,9 +56,8 @@ def densify_grids(pos: torch.Tensor, opacity: torch.Tensor, cov: torch.Tensor, g
     """densify_grids (filling.py:26-87): (count int32, density float32), both (grid_n, grid_n, grid_n), for Gaussians whose
     positions are already in the grid's frame."""
     _check_grid_n(grid_n)
-    lib = _lib.require_device()
-    if not (pos.is_cuda and opacity.is_cuda and cov.is_cuda):
-        raise _lib.PixieError("densify_grids requires CUDA tensors; there is no CPU fallback")
+    _lib.require_device()
+    _lib.require_cuda("densify_grids", pos, opacity, cov)
     p = pos.detach().reshape(-1, 3).to(torch.float32).contiguous()
     o = opacity.detach().reshape(-1).to(p.device, torch.float32).contiguous()
     c = cov.detach().reshape(-1, 6).to(p.device, torch.float32).contiguous()
@@ -70,11 +65,9 @@ def densify_grids(pos: torch.Tensor, opacity: torch.Tensor, cov: torch.Tensor, g
     if o.shape[0] != n or c.shape[0] != n:
         raise ValueError(f"pos, opacity and cov disagree on the Gaussian count ({n}, {o.shape[0]}, {c.shape[0]})")
     g = int(grid_n)
-    with torch.cuda.device(p.device):
-        count = torch.empty((g, g, g), dtype=torch.int32, device=p.device)
-        density = torch.empty((g, g, g), dtype=torch.float32, device=p.device)
-        _lib.check(lib.pixie_fill_density(C.c_void_p(p.data_ptr()), C.c_void_p(o.data_ptr()), C.c_void_p(c.data_ptr()), n, g, float(grid_dx),
-                                          C.c_void_p(count.data_ptr()), C.c_void_p(density.data_ptr()), _stream(p.device)))
+    count = torch.empty((g, g, g), dtype=torch.int32, device=p.device)
+    density = torch.empty((g, g, g), dtype=torch.float32, device=p.device)
+    _lib.call("pixie_fill_density", p.device, p, o, c, n, g, float(grid_dx), count, density)
     return count, density
 
 
@@ -89,21 +82,18 @@ def fill_grids(count: torch.Tensor, density: torch.Tensor, grid_dx: float, max_s
             raise ValueError(f"{name} must be in 0..5 ({_DIRS}), got {d}")
     if int(max_particles_per_cell) < 1:
         raise ValueError(f"max_particles_per_cell must be >= 1, got {max_particles_per_cell}")
-    lib = _lib.require_device()
-    if not (count.is_cuda and density.is_cuda):
-        raise _lib.PixieError("fill_grids requires CUDA tensors; there is no CPU fallback")
+    _lib.require_device()
+    _lib.require_cuda("fill_grids", count, density)
     g = count.shape[0]
     if count.dtype != torch.int32 or density.dtype != torch.float32 or tuple(count.shape) != (g, g, g) or density.shape != count.shape \
             or not count.is_contiguous() or not density.is_contiguous():
         raise ValueError("count / density must be contiguous (n, n, n) int32 / float32 grids")
     dev = count.device
     n_dense, n_total = C.c_int(0), C.c_int(0)
-    with torch.cuda.device(dev):
-        out = torch.empty((max(int(max_samples), 0), 3), dtype=torch.float32, device=dev)
-        _lib.check(lib.pixie_fill_grids(C.c_void_p(count.data_ptr()), C.c_void_p(density.data_ptr()), g, float(grid_dx),
-                                        (C.c_float * 3)(*[float(v) for v in origin]), float(density_thres), float(search_thres),
-                                        int(max_particles_per_cell), int(search_exclude_dir), int(ray_cast_dir), int(seed) & (2 ** 64 - 1),
-                                        C.c_void_p(out.data_ptr()), int(max_samples), C.byref(n_dense), C.byref(n_total), _stream(dev)))
+    out = torch.empty((max(int(max_samples), 0), 3), dtype=torch.float32, device=dev)
+    _lib.call("pixie_fill_grids", dev, count, density, g, float(grid_dx), (C.c_float * 3)(*[float(v) for v in origin]),
+              float(density_thres), float(search_thres), int(max_particles_per_cell), int(search_exclude_dir), int(ray_cast_dir),
+              int(seed) & (2 ** 64 - 1), out, int(max_samples), C.byref(n_dense), C.byref(n_total))
     return out[:n_total.value], n_dense.value
 
 
@@ -128,8 +118,7 @@ def fill_particles(pos: torch.Tensor, opacity: torch.Tensor, cov: torch.Tensor, 
         raise ValueError(f"opacity must hold N and cov N x 6 values for N = {n} Gaussians, got {tuple(opacity.shape)} and {tuple(cov.shape)}")
     if boundary is not None and len(boundary) != 6:
         raise ValueError("boundary must be [x0, x1, y0, y1, z0, z1]")
-    if not (pos.is_cuda and opacity.is_cuda and cov.is_cuda):
-        raise _lib.PixieError("fill_particles requires CUDA tensors; there is no CPU fallback")
+    _lib.require_cuda("fill_particles", pos, opacity, cov)
     pos_clone = pos.detach().to(torch.float32).clone()
     p, o, c = pos_clone, opacity.detach().reshape(-1), cov.detach().reshape(-1, 6)
     origin = (0.0, 0.0, 0.0)
@@ -154,18 +143,15 @@ def fill_particles(pos: torch.Tensor, opacity: torch.Tensor, cov: torch.Tensor, 
 def nearest_gaussian(pos: torch.Tensor, query: torch.Tensor) -> torch.Tensor:
     """The search of get_attr_from_closest (filling.py:383-405): (M,) int32, for each query the index of the Gaussian at
     the smallest float32 distance (ties to the lowest index), or -1 when none is closer than 1e10. Exact, on the device."""
-    lib = _lib.require_device()
-    if not (pos.is_cuda and query.is_cuda):
-        raise _lib.PixieError("nearest_gaussian requires CUDA tensors; there is no CPU fallback")
+    _lib.require_device()
+    _lib.require_cuda("nearest_gaussian", pos, query)
     if pos.dim() != 2 or pos.shape[1] != 3 or query.dim() != 2 or query.shape[1] != 3:
         raise ValueError(f"pos and query must be (N, 3) and (M, 3), got {tuple(pos.shape)} and {tuple(query.shape)}")
     dev = query.device
     p = pos.detach().to(dev, torch.float32).contiguous()
     q = query.detach().to(torch.float32).contiguous()
-    with torch.cuda.device(dev):
-        index = torch.empty(q.shape[0], dtype=torch.int32, device=dev)
-        _lib.check(lib.pixie_nearest_gaussian(C.c_void_p(p.data_ptr()), p.shape[0], C.c_void_p(q.data_ptr()), q.shape[0],
-                                              C.c_void_p(index.data_ptr()), _stream(dev)))
+    index = torch.empty(q.shape[0], dtype=torch.int32, device=dev)
+    _lib.call("pixie_nearest_gaussian", dev, p, p.shape[0], q, q.shape[0], index)
     return index
 
 
@@ -185,8 +171,7 @@ def init_filled_particles(pos: torch.Tensor, shs: torch.Tensor, cov: torch.Tenso
         raise ValueError(f"opacity must hold N and cov N x 6 values for N = {n} Gaussians, got {tuple(opacity.shape)} and {tuple(cov.shape)}")
     if new_pos.dim() != 2 or new_pos.shape[1] != 3:
         raise ValueError(f"new_pos must be (M, 3), got {tuple(new_pos.shape)}")
-    if not (pos.is_cuda and shs.is_cuda and cov.is_cuda and opacity.is_cuda and new_pos.is_cuda):
-        raise _lib.PixieError("init_filled_particles requires CUDA tensors; there is no CPU fallback")
+    _lib.require_cuda("init_filled_particles", pos, shs, cov, opacity, new_pos)
     dev = pos.device
     s = shs.detach().to(dev, torch.float32)
     o = opacity.detach().to(dev, torch.float32).reshape(n, 1)

@@ -141,7 +141,7 @@ def decode_checkpoint_ply(path: str, sh_degree: int = 3, opacity_threshold: Opti
     """pos (M, 3), shs (M, K, 3), opacity (M, 1) and cov (M, 6) of a Gaussian checkpoint PLY, decoded on the device; with
     `opacity_threshold`, only the rows whose opacity is > float32(threshold), in file order (gs_simulation.py:405)."""
     el, K, cols = _checkpoint_layout(path, sh_degree)
-    lib = _lib.require_device()
+    _lib.require_device()
     dev = torch.device(device)
     n, stride = el.count, el.dtype.itemsize
     pos = torch.empty((n, 3), dtype=torch.float32, device=dev)
@@ -151,12 +151,8 @@ def decode_checkpoint_ply(path: str, sh_degree: int = 3, opacity_threshold: Opti
     table = _checkpoint_table(el, dev)
     thr = 0.0 if opacity_threshold is None else float(np.float32(opacity_threshold))
     m = C.c_longlong(0)
-    with torch.cuda.device(dev):
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(lib.pixie_gaussian_checkpoint_decode(C.c_void_p(table.data_ptr()), n, stride, (C.c_int * len(cols))(*cols), K,
-                                                        int(opacity_threshold is not None), thr, C.c_void_p(pos.data_ptr()),
-                                                        C.c_void_p(shs.data_ptr()), C.c_void_p(opacity.data_ptr()), C.c_void_p(cov.data_ptr()),
-                                                        C.byref(m), stream))
+    _lib.call("pixie_gaussian_checkpoint_decode", dev, table, n, stride, (C.c_int * len(cols))(*cols), K, int(opacity_threshold is not None),
+              thr, pos, shs, opacity, cov, C.byref(m))
     table.record_stream(torch.cuda.current_stream(dev))
     M = m.value
     return {"pos": pos[:M], "shs": shs[:M], "opacity": opacity[:M], "cov": cov[:M]}
@@ -168,18 +164,15 @@ def decode_checkpoint_ply_scale_rot(path: str, sh_degree: int = 3, device="cuda:
     get_rotation (F.normalize, w x y z as stored) give them: what gaussian-splatting's render.py rasterizes. No opacity
     filter; the same pinned read and single host-to-device copy as decode_checkpoint_ply."""
     el, K, cols = _checkpoint_layout(path, sh_degree)
-    lib = _lib.require_device()
+    _lib.require_device()
     dev = torch.device(device)
     n, stride = el.count, el.dtype.itemsize
     table = _checkpoint_table(el, dev)
     out = {"pos": torch.empty((n, 3), dtype=torch.float32, device=dev), "shs": torch.empty((n, K, 3), dtype=torch.float32, device=dev),
            "opacity": torch.empty((n, 1), dtype=torch.float32, device=dev), "scales": torch.empty((n, 3), dtype=torch.float32, device=dev),
            "rotations": torch.empty((n, 4), dtype=torch.float32, device=dev)}
-    with torch.cuda.device(dev):
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(lib.pixie_gaussian_checkpoint_decode_scale_rot(
-            C.c_void_p(table.data_ptr()), n, stride, (C.c_int * len(cols))(*cols), K,
-            *(C.c_void_p(out[k].data_ptr()) for k in ("pos", "shs", "opacity", "scales", "rotations")), stream))
+    _lib.call("pixie_gaussian_checkpoint_decode_scale_rot", dev, table, n, stride, (C.c_int * len(cols))(*cols), K,
+              *(out[k] for k in ("pos", "shs", "opacity", "scales", "rotations")))
     table.record_stream(torch.cuda.current_stream(dev))
     return out
 

@@ -13,7 +13,6 @@ device. The query embeddings are an input: `--query_embeddings` (P, C), or the u
 from __future__ import annotations
 
 import argparse
-import ctypes as C
 import json
 import os
 from typing import Dict, List, Optional, Sequence
@@ -32,14 +31,6 @@ TAB10 = [tuple(int(h[i:i + 2], 16) / 255 for i in (1, 3, 5)) + (1.0,) for h in
          ("#1f77b4", "#ff7f0e", "#2ca02c", "#d62728", "#9467bd", "#8c564b", "#e377c2", "#7f7f7f", "#bcbd22", "#17becf")]
 SEGMENTED_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"), ("blue", "u1"), ("alpha", "u1"),
                             ("part_label", "<i4"), ("density", "<f4"), ("E", "<f4"), ("nu", "<f4"), ("material_id", "<i4")])
-
-
-def _ptr(t: Optional[torch.Tensor]):
-    return C.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream(device) -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 def str2bool(v):
@@ -73,7 +64,7 @@ def part_similarity(features: torch.Tensor, unit_queries: torch.Tensor, softmax_
     float16 `features` (..., C) selected by `mask` (over the leading dims, C order, any non-zero entry as in `mask.bool()`;
     every row without one).
     `unit_queries` (P, C) fp32 are normalize_queries' rows. `n_occupied` is mask's count when the caller has it."""
-    lib = _lib.require_device()
+    _lib.require_device()
     if not features.is_cuda or features.dtype != torch.float16:
         raise _lib.PixieError("part_similarity needs float16 CUDA features; there is no CPU fallback")
     C_ = features.shape[-1]
@@ -99,9 +90,7 @@ def part_similarity(features: torch.Tensor, unit_queries: torch.Tensor, softmax_
     scores = torch.empty(n, dtype=torch.float32, device=dev)
     # torch divides by a Python scalar as a multiplication by its fp32 reciprocal
     inv_t = float(np.float32(1.0) / np.float32(softmax_temperature))
-    with torch.cuda.device(dev):
-        _lib.check(lib.pixie_part_similarity(_ptr(f), _ptr(m8), f.shape[0], C_, n, _ptr(q), P, inv_t, _ptr(sims), _ptr(labels),
-                                             _ptr(scores), _ptr(probs), _stream(dev)))
+    _lib.call("pixie_part_similarity", dev, f, m8, f.shape[0], C_, n, q, P, inv_t, sims, labels, scores, probs)
     return sims, labels, scores, probs
 
 
@@ -117,15 +106,14 @@ def knn_label_vote(coords: torch.Tensor, labels: torch.Tensor, k: int = 200) -> 
     if not 1 <= k <= n:
         raise ValueError(f"Expected n_neighbors <= n_samples_fit, but n_neighbors = {k}, n_samples_fit = {n}, n_samples = {n}"
                          if k > n else f"k must be >= 1, got {k}")
-    lib = _lib.require_device()
+    _lib.require_device()
     dev = coords.device if coords.is_cuda else torch.device("cuda", torch.cuda.current_device())
     pos = coords.to(dev, torch.float32).contiguous()
     if not bool(torch.isfinite(pos).all()):
         raise ValueError("knn_label_vote needs finite coordinates")
     lab = labels.to(dev, torch.int64).contiguous()
     out = torch.empty(n, dtype=torch.int64, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.pixie_knn_label_vote(_ptr(pos), n, _ptr(lab), int(k), _ptr(out), _stream(dev)))
+    _lib.call("pixie_knn_label_vote", dev, pos, n, lab, int(k), out)
     return out
 
 
@@ -136,13 +124,12 @@ def nearest_vertex(vertices: np.ndarray, queries: torch.Tensor) -> torch.Tensor:
     vertices = np.ascontiguousarray(vertices, dtype=np.float64)
     if vertices.ndim != 2 or vertices.shape[1] != 3 or queries.ndim != 2 or queries.shape[1] != 3:
         raise ValueError(f"vertices and queries must be (n, 3) and (m, 3), got {vertices.shape} and {tuple(queries.shape)}")
-    lib = _lib.require_device()
+    _lib.require_device()
     dev = queries.device if queries.is_cuda else torch.device("cuda", torch.cuda.current_device())
     v = torch.from_numpy(vertices).to(dev)
     q = queries.to(dev, torch.float32).contiguous()
     idx = torch.empty(q.shape[0], dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.pixie_nearest_vertex(_ptr(v), v.shape[0], _ptr(q), q.shape[0], _ptr(idx), _stream(dev)))
+    _lib.call("pixie_nearest_vertex", dev, v, v.shape[0], q, q.shape[0], idx)
     return idx.cpu().to(torch.int64)
 
 

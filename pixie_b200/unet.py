@@ -182,7 +182,7 @@ class _B200UNet:
             try:
                 for k, v in self._state.items():
                     shape = (C.c_int64 * v.dim())(*v.shape)
-                    _lib.check(lib.pixie_unet_set_tensor(h, k.encode(), C.c_void_p(v.data_ptr()), shape, v.dim()))
+                    _lib.check(lib.pixie_unet_set_tensor(h, k.encode(), _lib.ptr(v), shape, v.dim()))
                 _lib.check(lib.pixie_unet_finalize(h))
             except Exception:
                 lib.pixie_unet_destroy(h)
@@ -215,11 +215,10 @@ class _B200UNet:
         n = x.shape[0]
         out = torch.empty((n, self.out_channels, G, G, G), dtype=torch.float32, device=self._device)
         with torch.cuda.device(self._device):
-            st = torch.cuda.current_stream().cuda_stream
+            st = _lib.stream(self._device)
             for b0 in range(0, n, self.max_batch):
                 nb = min(self.max_batch, n - b0)
-                _lib.check(lib.pixie_unet_forward_ncdhw(self._handle, C.c_void_p(x[b0:b0 + nb].data_ptr()), nb,
-                                                        C.c_void_p(out[b0:b0 + nb].data_ptr()), C.c_void_p(st)))
+                _lib.check(lib.pixie_unet_forward_ncdhw(self._handle, _lib.ptr(x[b0:b0 + nb]), nb, _lib.ptr(out[b0:b0 + nb]), st))
         return out
 
     def forward_channels_last_f16(self, feat_ndhwc: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -239,11 +238,10 @@ class _B200UNet:
         elif tuple(out.shape) != (n, self.out_channels, G, G, G) or out.dtype != torch.float32 or not out.is_contiguous():
             raise ValueError("out must be a contiguous float32 (N, out_channels, D, H, W) device tensor")
         with torch.cuda.device(self._device):
-            st = torch.cuda.current_stream().cuda_stream
+            st = _lib.stream(self._device)
             for b0 in range(0, n, self.max_batch):
                 nb = min(self.max_batch, n - b0)
-                _lib.check(lib.pixie_unet_forward(self._handle, C.c_void_p(x[b0:b0 + nb].data_ptr()), nb,
-                                                  C.c_void_p(out[b0:b0 + nb].data_ptr()), C.c_void_p(st)))
+                _lib.check(lib.pixie_unet_forward(self._handle, _lib.ptr(x[b0:b0 + nb]), nb, _lib.ptr(out[b0:b0 + nb]), st))
         return out
 
     def forward_host(self, feat_ndhwc_pinned: torch.Tensor, out_pinned: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -258,9 +256,8 @@ class _B200UNet:
         if out_pinned is None:
             out_pinned = torch.empty((n, self.out_channels, G, G, G), dtype=torch.float32).pin_memory()
         with torch.cuda.device(self._device):
-            st = torch.cuda.current_stream().cuda_stream
-            _lib.check(lib.pixie_unet_forward_host(self._handle, C.c_void_p(feat_ndhwc_pinned.data_ptr()), n,
-                                                   C.c_void_p(out_pinned.data_ptr()), C.c_void_p(st)))
+            _lib.check(lib.pixie_unet_forward_host(self._handle, _lib.ptr(feat_ndhwc_pinned), n, _lib.ptr(out_pinned),
+                                                   _lib.stream(self._device)))
         return out_pinned
 
     # ---- introspection used by bench/tests --------------------------------------------------------
@@ -285,9 +282,7 @@ class _B200UNet:
         cap = 1024
         ms, kinds, fl = (C.c_float * cap)(), (C.c_int * cap)(), (C.c_double * cap)()
         with torch.cuda.device(self._device):
-            st = torch.cuda.current_stream().cuda_stream
-            k = lib.pixie_unet_profile(self._handle, C.c_void_p(feat_ndhwc.data_ptr()), n, C.c_void_p(out.data_ptr()),
-                                       C.c_void_p(st), ms, kinds, fl, cap)
+            k = lib.pixie_unet_profile(self._handle, _lib.ptr(feat_ndhwc), n, _lib.ptr(out), _lib.stream(self._device), ms, kinds, fl, cap)
         if k < 0:
             raise _lib.last_error()
         names = {0: "conv", 1: "moments", 2: "norm", 3: "upsample", 4: "attention"}
@@ -296,7 +291,7 @@ class _B200UNet:
     def debug_fetch(self, name: str, channels: int, sp: int, batch: int = 1) -> torch.Tensor:
         """Intermediate activation by reference module path, returned as (N, C, D, H, W) fp32 (CPU)."""
         buf = torch.empty(batch * sp ** 3 * channels, dtype=torch.float32)
-        n = _lib.load().pixie_unet_debug_fetch(self._handle, name.encode(), C.c_void_p(buf.data_ptr()), buf.numel())
+        n = _lib.load().pixie_unet_debug_fetch(self._handle, name.encode(), _lib.ptr(buf), buf.numel())
         if n < 0:
             raise _lib.last_error()
         return buf[:n].view(batch, sp, sp, sp, channels).permute(0, 4, 1, 2, 3).contiguous()

@@ -69,7 +69,7 @@ def main():
         cams = [D.loadCam(-1, info)[0] for info in train[:20]]
         for cam in cams:
             ms = [0.0] * 5
-            GR._rasterize_scale_rot(g["pos"], g["scales"], g["rotations"], g["opacity"], cam, bg, g["shs"], 3, phase_ms=ms)
+            GR._rasterize(g["pos"], g["opacity"], cam, bg, g["shs"], 3, scales=g["scales"], rotations=g["rotations"], phase_ms=ms)
             phases.append(ms)
         p = np.mean(np.array(phases), 0)
         out["device_ms_per_view"] = {"preprocess": p[0], "sort": p[1] + p[2] + p[3], "blend": p[4], "total": float(p.sum())}

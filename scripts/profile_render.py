@@ -66,7 +66,7 @@ def main():
                 t_ours.append(timed(ours))
                 t_ref.append(timed(ref))
                 ph = [0.0] * 5
-                _, _, pairs = GR._rasterize(pos, cov, op, cam, [0, 0, 0], shs=shs, sh_degree=3, phase_ms=ph)
+                _, _, pairs = GR._rasterize(pos, op, cam, [0, 0, 0], shs=shs, sh_degree=3, cov3D=cov, phase_ms=ph)
                 phases.append(ph)
             ph = np.median(np.array(phases), axis=0)
             img, _ = ours()

@@ -3,6 +3,7 @@ the fp64 brute-force rasterizer (oracle/gs_render_ref.py) against closed forms, 
 reference's rasterizer binary (built into oracle/_ref/ by oracle/build_gs_rasterizer_ref.py) and the oracle."""
 from __future__ import annotations
 
+import dataclasses
 import importlib.machinery
 import importlib.util
 import json
@@ -217,6 +218,21 @@ def test_capi_symbols_present(built_lib):
         assert hasattr(built_lib, name)
 
 
+def test_capi_render_takes_one_covariance_source(built_lib):
+    """cov_dev, or scales_dev and rotations_dev with shs_dev: other combinations are refused before anything is read."""
+    import ctypes as C
+    f3, f16 = (C.c_float * 3)(), (C.c_float * 16)()
+    dummy = C.c_void_p(16)
+
+    def render(cov, scales, rotations, shs, colors):
+        return built_lib.pixie_gs_render(None, dummy, cov, scales, rotations, dummy, shs, 16, 3, colors, 1, f16, f16, f3, 1.0, 1.0,
+                                         4, 4, f3, dummy, dummy, None, None, None)
+    assert render(dummy, dummy, dummy, dummy, None) != 0
+    assert b"not both" in built_lib.pixie_last_error()
+    assert render(None, dummy, dummy, None, dummy) != 0
+    assert b"colors_dev needs cov_dev" in built_lib.pixie_last_error()
+
+
 def test_rasterize_argument_validation():
     cam = _simple_cam(16, 16)
     n = 4
@@ -239,6 +255,30 @@ def test_rasterize_argument_validation():
     from pixie_b200 import _lib
     with pytest.raises(_lib.PixieError, match="CPU fallback"):
         GR.rasterize(m, c, o, cam, [0, 0, 0], shs=shs, sh_degree=3)
+
+
+def test_rasterize_scale_rot_argument_validation():
+    cam = _simple_cam(16, 16)
+    n = 4
+    m, sc, rot, o = torch.zeros(n, 3), torch.ones(n, 3), torch.zeros(n, 4), torch.ones(n)
+    shs = torch.zeros(n, 16, 3)
+    bad = [
+        (dict(means3D=torch.zeros(n, 4)), "means3D must be"),
+        (dict(scales=torch.ones(n, 4)), "scales must be"),
+        (dict(rotations=torch.zeros(n, 3)), "rotations must be"),
+        (dict(opacity=torch.ones(n, 2)), "opacity must be"),
+        (dict(sh_degree=4), "sh_degree must be"),
+        (dict(shs=torch.zeros(n, 4, 3), sh_degree=2), "shs must be"),
+        (dict(camera=dataclasses.replace(cam, image_width=0)), "image size"),
+    ]
+    for b, msg in bad:
+        kw = dict(means3D=m, scales=sc, rotations=rot, opacity=o, camera=cam, bg=[0, 0, 0], shs=shs, sh_degree=3)
+        kw.update(b)
+        with pytest.raises(ValueError, match=msg):
+            GR.rasterize_scale_rot(**kw)
+    from pixie_b200 import _lib
+    with pytest.raises(_lib.PixieError, match="rasterize_scale_rot requires CUDA tensors; there is no CPU fallback"):
+        GR.rasterize_scale_rot(m, sc, rot, o, cam, [0, 0, 0], shs, 3)
 
 
 def test_scene_defaults_leave_rendering_off():
